@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — DiT-step latent tokens/s of the B200-native miniFLUX sampler step (BASELINE.json metric).
+"""bench.py — DiT-step latent tokens/s of the CUDA-native miniFLUX sampler step (BASELINE.json metric).
 
 A "step" is ONE DiT forward (the pipeline's `self.dit(...)` call, P:760-766) at the headline single-step shape of the
 768p / 10 s configuration (BASELINE.md §2): unit 30, stage 2 — CFG batch B=2, S = 128 text + 28x240 + 960 + 3840 history
@@ -10,12 +10,13 @@ memory; strong scaling, `parity_vs_n1` = max |sharded - single-GPU| of the step'
 The line also carries the second half of BASELINE's metric: `vae_decode` (768p causal-VAE decode, frames/s + conv roofline)
 and `video_e2e` (the whole 768p / 10 s pyramidal sampler + decode, frames/s), and two baselines timed in the same run: the
 reference algorithm on the host cores (`cpu_baseline`) and the UNMODIFIED reference modules in eager PyTorch bf16 on the
-same B200 (`gpu_eager_baseline`, from the copy staged in baseline/_ref).
+same GPU (`gpu_eager_baseline`, from the copy staged in oracle/_ref).
 
   python bench.py [--gpus N] [--steps K] [--warmup W]           our arm (CUDA kernels through the C-ABI)
+  python bench.py ... --dump-outputs DIR                         also writes the last timed step's output as DIR/<name>.npy
   python bench.py --impl reference ...                           the reference algorithm's CPU path (oracle port), host cores
 
-Prints ONE JSON line (rank 0).  See DESIGN.md §Measurement for the definitions of value / e2e / roofline / cpu_baseline.
+Prints ONE JSON line (rank 0).  DESIGN.md defines value / e2e / roofline / cpu_baseline.
 """
 from __future__ import annotations
 
@@ -31,7 +32,6 @@ from pathlib import Path
 ROOT = Path(__file__).resolve().parent
 sys.path.insert(0, str(ROOT))
 
-ATTN_TRAFFIC_BYTES = 460.71e6   # profiles/r02_attn2_final_ncu.txt: dram__bytes_read 358.04 MB + dram__bytes_write 102.67 MB per launch
 METRIC = "dit_step_latent_tokens_per_sec"
 UNIT = "tokens/s"
 WORKLOAD = ("miniFLUX 768p/10s (BASELINE configs[2]) — one DiT forward at unit 30 / stage 2: CFG batch 2, "
@@ -50,7 +50,7 @@ def cpu_sample_clip_shapes(batch=2):
 
 # ----------------------------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -97,12 +97,8 @@ class ClockSampler:
 
 
 def measured_peaks():
-    p = ROOT / "MEASURED_PEAKS.json"
-    if p.exists():
-        d = json.loads(p.read_text())
-        return {"tflops_sustained": d.get("bf16_tflops_sustained"), "tflops_burst": d.get("bf16_tflops"),
-                "hbm_gbs": d.get("hbm_gbs"), "source": "measured (MEASURED_PEAKS.json)"}
-    return {"tflops_sustained": 1400.0, "tflops_burst": 1590.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"tflops_sustained": 989.0, "tflops_burst": 989.0, "hbm_gbs": 3350.0,
+            "source": "NVIDIA data sheet, H100 SXM at 700 W (dense bf16, HBM3); not a measured rate"}
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -111,7 +107,7 @@ def cpu_reference_sample(n_double=1, n_single=2, threads=None, repeats=1):
     the full 8+16-block forward, and a description of the sample."""
     import torch
     from oracle import flux_oracle as FO
-    # every host core, whatever the launcher exported (torchrun sets OMP_NUM_THREADS=1: round 1's N>1 CPU arm ran on one thread)
+    # every host core, whatever the launcher exported (torchrun sets OMP_NUM_THREADS=1)
     torch.set_num_threads(threads or os.cpu_count() or 1)
     threads = torch.get_num_threads()
     cfg = FO.FluxConfig(num_layers=n_double, num_single_layers=n_single)
@@ -169,14 +165,14 @@ def run_reference(args):
 
 
 def gpu_eager_reference(dev, host, steps=2):
-    """The UNMODIFIED reference `PyramidFluxTransformer` (baseline/_ref copy through oracle/pin/ref_shim.py) in eager PyTorch
+    """The UNMODIFIED reference `PyramidFluxTransformer` (oracle/_ref copy through oracle/pin/ref_shim.py) in eager PyTorch
     under bf16 autocast on this GPU: the full 8+16-block forward at the bench shape, dense [B,1,S,S] bool mask + SDPA as the
-    reference builds them (F:318-350, B:363-365).  A reported baseline (SURVEY.md §8d), never on the product path."""
+    reference builds them (F:318-350, B:363-365).  A reported baseline, never on the product path."""
     import torch
     try:
         from oracle.pin import ref_shim
         if not ref_shim.reference_available():
-            return {"unavailable": "reference packages not staged in baseline/_ref (oracle/pin/stage_reference.py)"}
+            return {"unavailable": "reference packages not staged in oracle/_ref (oracle/pin/stage_reference.py)"}
         ref_shim.install()
         from pyramid_dit.flux_modules import PyramidFluxTransformer
         with torch.device(dev):
@@ -363,13 +359,15 @@ def run_mmdit(args):
                   pooled_projections=host["pooled"].to(dev, non_blocking=True))[0]
         out_host.copy_(o, non_blocking=True)
 
+    last = {}
+
     def timed(fn, steps):
         torch.cuda.synchronize()
         s_, e_ = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         n0 = _lib.launch_count()
         s_.record()
         for _ in range(steps):
-            fn()
+            last["out"] = fn()
         e_.record()
         torch.cuda.synchronize()
         return s_.elapsed_time(e_) / steps, _lib.launch_count() - n0
@@ -383,6 +381,8 @@ def run_mmdit(args):
     ms, launches = timed(step_resident, args.steps)
     t1 = time.time()
     clocks = sampler.stop(t0, t1)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"velocity": last["out"]})
     step_e2e()
     ms_e2e, _ = timed(step_e2e, args.steps)
     plan = model.last_plan
@@ -400,7 +400,7 @@ def run_mmdit(args):
             "config": {"workload": ("SD3 MMDiT 768p/5s (BASELINE configs[4]) — one DiT forward at unit 15 / stage 2: CFG batch 2, "
                                     "S=11888 (128 text + 13x240 + 960 + 3840 history + 3840 current), 24 joint blocks, D=1536, 24 heads"),
                        "global_batch": b, "seq_len": plan.seq, "parallelism": "single GPU", "launch_mode": "host-launched",
-                       "l2": "per-step working set exceeds the 126 MB L2; no explicit flush",
+                       "l2": "per-step working set exceeds the 50 MB L2; no explicit flush",
                        "step_tflop": {"gemm": gemm / 1e12, "attention_masked": attn / 1e12}},
             "clocks": clocks,
             "e2e": {"value": tokens / (ms_e2e * 1e-3), "unit": UNIT, "ms_per_step": ms_e2e, "h2d_bytes_per_step": h2d,
@@ -417,7 +417,7 @@ def run_mmdit(args):
 def vae_decode_leg(dev, world, rank):
     """Causal-VAE decode at 768p (BASELINE configs[2], second half of the metric): un-tiled, temporally chunked (window 4),
     5 latent -> 33 video frames on one GPU; with N GPUs 1 + 4 N latent frames, context-parallel (temporal split + 2-frame
-    halo exchange per causal conv).  Conv roofline: 1.10e7 MAC per output pixel-frame (SURVEY.md §8a) against the measured
+    halo exchange per causal conv).  Conv roofline: 1.10e7 MAC per output pixel-frame against the
     sustained bf16 peak."""
     import torch
     from pyramid_flow_b200.vae import B200CausalVAE, VaeConfigB200
@@ -464,7 +464,7 @@ def vae_decode_leg(dev, world, rank):
 
 def video_e2e_leg(dit, dev, world, rank):
     """frames/s end to end at 768p / 10 s (temp 31 -> 241 frames): the 3-stage pyramidal sampler loop (960 DiT calls, steps
-    20/10, CFG) + causal-VAE decode, text embeddings synthetic (text encoding excluded as SURVEY.md §8d defines).  Every rank
+    20/10, CFG) + causal-VAE decode, text embeddings synthetic (text encoding excluded).  Every rank
     runs the same loop; the DiT step is CFG x SP sharded, the decode context-parallel."""
     import torch
     from pyramid_flow_b200.sampler import B200PyramidSampler
@@ -503,20 +503,32 @@ def video_e2e_leg(dit, dev, world, rank):
         lat_n = lat.clone()
         lat_n[:, :, :1] = lat_n[:, :, :1] / sampler.vae_scale_factor + sampler.vae_shift_factor
         lat_n[:, :, 1:] = lat_n[:, :, 1:] / sampler.vae_video_scale_factor + sampler.vae_video_shift_factor
-        img = vae.decode(lat_n, temporal_chunk=True, window_size=4).sample
+        # 241 frames at 768p next to the resident DiT: chunks of 2 latent frames (the decoder's default window) and the
+        # sampler's cached blocks handed back first keep the decode inside an 80 GB card
+        torch.cuda.empty_cache()
+        img = vae.decode(lat_n, temporal_chunk=True, window_size=2).sample
         u8 = img.float().mul(127.5).add(127.5).clamp(0, 255).byte().permute(0, 2, 3, 4, 1).contiguous().cpu()
         torch.cuda.synchronize()
         t2 = time.time()
     finally:
         dit.forward = orig
     frames = 241
-    res = {"config": "miniFLUX 768x1280, temp=31 (241 frames), steps 20/10, guidance 7/5, un-tiled decode (window 4)",
+    res = {"config": "miniFLUX 768x1280, temp=31 (241 frames), steps 20/10, guidance 7/5, un-tiled decode (window 2)",
            "frames_per_s_end_to_end": frames / (t2 - t0), "seconds": t2 - t0, "dit_seconds": t1 - t0,
            "decode_seconds": t2 - t1, "dit_calls": sampler.dit_calls, "dit_token_passes_per_s": tokens[0] / (t1 - t0),
            "video_shape": list(u8.shape), "latent_finite": bool(torch.isfinite(lat.float()).all())}
     del vae, img, u8
     torch.cuda.empty_cache()
     return res
+
+
+def dump_outputs(directory, arrays):
+    """What the timed path returned in its last timed step, one float32 .npy per name (the inputs are seeded: two builds run with
+    the same arguments can be compared output for output)."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(directory, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 def run_ours(args):
@@ -541,10 +553,6 @@ def run_ours(args):
     model = B200FluxTransformer(cfg, sd, device=dev)
     del sd
     torch.cuda.empty_cache()
-    if args.attn_variant is not None:
-        model.attn_variant = args.attn_variant
-    if args.attn_phase is not None:
-        _lib.set_option(_lib.PF_OPT_ATTN_TILE_PHASE, args.attn_phase)
     lay = None
     b = 2
     g = torch.Generator().manual_seed(100)
@@ -609,7 +617,7 @@ def run_ours(args):
         s.record()
         h0 = time.perf_counter()
         for _ in range(steps):
-            fn()
+            host_ms["out"] = fn()
         host_ms["last"] = (time.perf_counter() - h0) * 1e3 / steps     # host time to ENQUEUE a step (no sync inside)
         e.record()
         barrier()
@@ -634,6 +642,8 @@ def run_ours(args):
     host_enqueue_ms = host_ms["last"]
     t1 = time.time()
     clocks = sampler.stop(t0, t1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"velocity": host_ms["out"]})
     # the timed region above carries no per-launch instrumentation (graph replay, or plain host launches with --no-graph);
     # the dominant kernel's launch durations come from the same number of host-launched steps run right after it, with CUDA
     # events around each attention launch
@@ -693,10 +703,7 @@ def run_ours(args):
     h2d = sum(x.numel() * x.element_size() for x in host["clips"]) + sum(
         host[k].numel() * host[k].element_size() for k in ("enc", "mask", "pooled", "t"))
     d2h = out_host.numel() * out_host.element_size()
-    # which attention kernel the step launched: the three-q-tile kernel unless the launches carry peer stores (SP > 1)
-    triple = bool(_lib.get_option(_lib.PF_OPT_ATTN_TRIPLE_KERNEL)) and (lay is None or lay.sp == 1) and args.attn_variant in (None, 0, 0x20)
-    attn_kernel_name = ("pf::attn3q_fwd_kernel (masked joint attention, three q tiles per CTA, 64-column kv steps, tcgen05)" if triple
-                        else "pf::attn2_fwd_kernel (masked joint attention, two q tiles per CTA, tcgen05)")
+    attn_kernel_name = "pf::attn_fwd_kernel (masked joint attention, one 128-row q tile per CTA, wgmma)"
     line = {
         "metric": METRIC, "value": tokens / (ms_step * 1e-3), "unit": UNIT, "n_gpus": world,
         "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms_step, "higher_is_better": True,
@@ -708,7 +715,7 @@ def run_ours(args):
                                    ("remote stores fused into the QKV-GEMM / attention epilogues over NVLink peer memory + "
                                     "flag barriers, no NCCL call in the step" if args.exchange == "peer" else
                                     "NCCL all_to_all_single each side of attention")),
-                   "layers": list(args.layers), "l2": "per-step working set (>1.5 GB of activations + 3.9 GB weights) exceeds the 126 MB L2; no explicit flush",
+                   "layers": list(args.layers), "l2": "per-step working set (>1.5 GB of activations + 3.9 GB weights) exceeds the 50 MB L2; no explicit flush",
                    "step_tflop": {"gemm": fl["gemm"] / 1e12, "attention_masked": fl["attention"] / 1e12},
                    "step_tflops_achieved": (fl["gemm"] + fl["attention"]) / (ms_step * 1e-3) / 1e12,
                    "launch_mode": ("CUDA graph replay of the step's launch sequence (captured once in warm-up), no per-launch "
@@ -728,15 +735,11 @@ def run_ours(args):
         "vae_decode": vae_leg, "video_e2e": video_leg, "gpu_eager_baseline": eager_leg,
         "roofline": {"kernel": attn_kernel_name, "bound": "tensor",
                      "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": (achieved / peak) if achieved else None,
-                     "peak_source": peaks["source"] + ", sustained cuBLAS bf16 (kernel timed inside a long step)",
+                     "peak_source": peaks["source"],
                      "launches_timed": len(attn_ms), "avg_launch_ms": attn_avg,
                      "share_of_step": (attn_avg * n_attn / ms_eager) if ms_eager else None,
                      "algorithmic_flops_per_launch": attn_flops_launch,
-                     # dram__bytes_read.sum + dram__bytes_write.sum of one `ncu --set full` capture of this kernel at this
-                     # shape (profiles/r02_attn2_final_ncu.txt) -- the algorithmic bytes are Q+K+V+O
-                     "traffic": ATTN_TRAFFIC_BYTES if (lay is None and not triple) else None, "traffic_unit": "B/launch",
-                     "traffic_note": ("no ncu capture of the three-q-tile kernel (GPU budget of the round spent); the two-q-tile "
-                                      "kernel at this shape: 460.7 MB = Q+K+V+O once (profiles/r02_attn2_final_ncu.txt)") if triple else None,
+                     "traffic": None, "traffic_unit": "B/launch", "traffic_note": "DRAM traffic not measured",
                      "algorithmic_bytes_per_launch": 4.0 * b * plan.seq * cfg.inner_dim * 2},
     }
     if args.no_cpu:
@@ -761,12 +764,14 @@ def main():
     ap.add_argument("--no-graph", action="store_true", help="(debug) launch every kernel from the host instead of replaying the captured CUDA graph")
     ap.add_argument("--model", default="flux", choices=["flux", "mmdit"], help="flux = miniFLUX (the headline, configs[2]); mmdit = SD3 MMDiT 768p/5s (configs[4])")
     ap.add_argument("--exchange", default=None, choices=["peer", "nccl"], help="N>1: peer-memory fused exchange (default) or NCCL all-to-all (A/B)")
-    ap.add_argument("--attn-variant", type=lambda x: int(x, 0), default=None, help="(debug) pf_attn_desc.variant of the DiT's attention launches")
-    ap.add_argument("--attn-phase", type=int, default=None, help="(debug) pf_set_option(PF_OPT_ATTN_TILE_PHASE, clocks)")
     ap.add_argument("--no-vae", action="store_true", help="skip the VAE decode leg")
     ap.add_argument("--no-video", action="store_true", help="skip the 768p/10s end-to-end sampler + decode leg (~1 min at N=1)")
     ap.add_argument("--no-eager", action="store_true", help="skip the reference-eager-on-GPU baseline leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned as DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the CUDA path's output; it cannot be combined with --impl reference")
     if args.impl == "reference":
         run_reference(args)
     elif args.model == "mmdit":

@@ -1,10 +1,10 @@
-/* pf_b200.h — C-ABI of libpf_b200.so: the sm_100a kernels behind the Pyramid-Flow sampler hot path.
+/* pf_b200.h — C-ABI of libpf_b200.so: the sm_90a (Hopper) kernels behind the Pyramid-Flow sampler hot path.
  *
- * Boundary contract (SURVEY.md §8b):
+ * Boundary contract:
  *   - plain C, raw device pointers + sizes + a cudaStream_t (passed as void*); no torch types;
  *   - every function returns 0 on success, <0 on error; pf_last_error() gives the message;
  *   - the caller owns every buffer; kernels are stream-ordered and hold no global mutable state;
- *   - there is NO CPU fallback: on a machine without an sm_100 GPU every compute entry fails.
+ *   - there is NO CPU fallback: on a machine without an sm_90 GPU every compute entry fails.
  *
  * Each entry cites the reference op site (file:line under jy0205/Pyramid-Flow @3040d71) it replaces.
  * Abbreviations: F = pyramid_dit/flux_modules/modeling_pyramid_flux.py, B = .../modeling_flux_block.py,
@@ -27,7 +27,7 @@ extern "C" {
 /* ------------------------------------------------------------------ misc */
 PF_API const char* pf_last_error(void);
 PF_API int pf_version(void);
-/* 0 if the current CUDA device is sm_100 (B200) and the driver exposes cuTensorMapEncodeTiled; <0 otherwise. */
+/* 0 if the current CUDA device is sm_90 (H100) and the driver exposes cuTensorMapEncodeTiled; <0 otherwise. */
 PF_API int pf_device_check(void);
 /* Loads every kernel instantiation of the library on the CURRENT device and sets its dynamic shared-memory attribute, so
  * that no later launch initialises anything host-side (required before capturing launches into a CUDA graph; also what makes
@@ -35,27 +35,27 @@ PF_API int pf_device_check(void);
 PF_API int pf_warmup(void);
 /* Library options: data-path choices that do not change results (same arithmetic, same bits) but are A/B-measured. */
 enum {
-  PF_OPT_GEMM_STAGED_RESID = 0, /* GATE_RESID epilogue: residual read-modify-write transposed through shared memory */
-  PF_OPT_GEMM_WAVE_TILING = 1,  /* wave-quantisation-aware tile width for GEMMs with few rows */
-  PF_OPT_ATTN_PAIR_KERNEL = 2,  /* variant 0 of pf_attn_fwd_masked = the two-q-tile kernel (needs pair_sched) */
-  PF_OPT_ATTN_TILE_PHASE = 3,   /* two-q-tile attention kernel: SM clocks the second q tile's softmax warps are held back once per
-                                 * CTA so the two tiles run out of phase (0 = start together) */
-  PF_OPT_ATTN_TRIPLE_KERNEL = 4, /* variant 0 of pf_attn_fwd_masked = the three-q-tile kernel when group_sched is given and the
-                                  * launch has no peer stores (the sequence-parallel path keeps the two-q-tile kernel: the
-                                  * three-q-tile kernel was validated on one GPU only) */
+  PF_OPT_GEMM_STAGED_RESID = 0, /* GATE_RESID epilogue: residual read-modify-write by whole row segments (a warp per row) instead
+                                 * of one thread per row */
+  PF_OPT_GEMM_WAVE_TILING = 1,  /* 64-wide column tiles when their wave count, costed at the measured 0.75 efficiency, beats 128-wide ones */
+  /* q-tile grouping hints of pf_attn_fwd_masked.  The sm_90a build has one attention kernel (one q tile per CTA, scores in
+   * registers); the three keys are accepted and stored so that existing callers keep working, and change nothing. */
+  PF_OPT_ATTN_PAIR_KERNEL = 2,
+  PF_OPT_ATTN_TILE_PHASE = 3,
+  PF_OPT_ATTN_TRIPLE_KERNEL = 4,
   PF_OPT_COUNT = 5
 };
 #define PF_OPT_DEFAULT_GEMM_STAGED_RESID 1
 #define PF_OPT_DEFAULT_GEMM_WAVE_TILING 1
 #define PF_OPT_DEFAULT_ATTN_PAIR_KERNEL 1
-#define PF_OPT_DEFAULT_ATTN_TRIPLE_KERNEL 1   /* measured on B200: 2.80 -> 2.60 ms per launch at the bench shape, whole GPU suite green with it */
-#define PF_OPT_DEFAULT_ATTN_TILE_PHASE 800   /* measured on B200: 2.84 -> 2.78 ms per launch at the bench shape (tools/gpu_check.py attn_phase_sweep) */
+#define PF_OPT_DEFAULT_ATTN_TRIPLE_KERNEL 1
+#define PF_OPT_DEFAULT_ATTN_TILE_PHASE 800
 PF_API int pf_set_option(int key, int value);
 PF_API int pf_get_option(int key);
 /* number of kernels launched by this library since load (bench.py's gpu_launches claim). */
 PF_API int64_t pf_launch_count(void);
 
-/* ------------------------------------------------------------------ step contexts (SURVEY.md §8b: pf_ctx_*, pf_dit_step_*)
+/* ------------------------------------------------------------------ step contexts (pf_ctx_*, pf_dit_step_*)
  * A pf_ctx owns ONE recorded launch sequence: between pf_ctx_record_begin and pf_ctx_record_end every pf_* launch issued on
  * `stream` by the calling thread is recorded instead of executed (descriptor validation, tensor-map encoding and kernel
  * selection happen once, at record time); pf_dit_step_flux / pf_dit_step_mmdit / pf_vae_decode_chunk then re-issue the whole
@@ -98,8 +98,8 @@ PF_API int pf_peer_barrier(const PfPeerGroup* grp, uint32_t* epoch_counter, void
 /* dst->ptr[i][dst_offset_bytes ...] = src[0 .. bytes) for every member (16-byte granularity). */
 PF_API int pf_peer_bcast(const PfPeerGroup* dst, const void* src, int64_t bytes, int64_t dst_offset_bytes, void* stream);
 
-/* ------------------------------------------------------------------ GEMM (tcgen05 + TMA)
- * out = epilogue(A[rows, K] . W[N, K]^T + bias).  bf16 operands, fp32 accumulation in TMEM.
+/* ------------------------------------------------------------------ GEMM (wgmma + TMA)
+ * out = epilogue(A[rows, K] . W[N, K]^T + bias).  bf16 operands, fp32 accumulation in registers.
  * Replaces every nn.Linear on the DiT path: x_embedder/context_embedder F:290,F:401; to_q/k/v, add_*_proj B:816-835;
  * to_out/to_add_out B:868-872; FeedForward B:73-100; proj_mlp/proj_out B:923-938; norm_out+proj_out F:538-539;
  * with the elementwise ops around them fused into the epilogue (bias, GELU-tanh, per-head RMSNorm N:66-79,
@@ -143,7 +143,7 @@ typedef struct pf_gemm_desc {
   float norm_eps;
   int32_t heads, head_dim, seq_len;
   int32_t n_split; /* QKV_GELU: first n_split (=3*H*hd) columns are q|k|v */
-  int32_t kernel_variant; /* 0 = auto (measured policy); 1 = force 1-CTA tiles; 2 = force 2-CTA (cta_group::2) tiles.
+  int32_t kernel_variant; /* 0 = auto; 1 = force 128-wide column tiles (n % 128 == 0); 2 = force 64-wide column tiles.
                            * Same bits either way (same K order); exists so tests can pin each kernel. */
   /* QKV_ROPE under sequence parallelism (peer_count > 1): head h of this rank's token chunk is stored into rank
    * (h / peer_heads)'s buffer peer_qkv[h / peer_heads], laid out [3 (q,k,v)][peer_heads][peer_seq][head_dim], at sequence
@@ -154,7 +154,7 @@ typedef struct pf_gemm_desc {
 
 PF_API int pf_gemm_bf16(const pf_gemm_desc* desc, void* stream);
 
-/* ------------------------------------------------------------------ masked joint attention (tcgen05 + TMA)
+/* ------------------------------------------------------------------ masked joint attention (wgmma + TMA)
  * softmax(Q K^T * scale + mask) V with mask(q, kv) = (seg[q] == seg[kv]) && (time[q] >= time[kv])  (F:318-350),
  * replacing F.scaled_dot_product_attention with the dense bool mask at B:363-365 and B:596-598.
  * q,k,v: bf16 [batch, heads, seq, 64]; out: bf16 [batch, seq, heads*64] with row stride ldo (elements).
@@ -172,20 +172,20 @@ typedef struct pf_attn_desc {
   const int32_t* time;       /* device [batch, seq] */
   const int32_t* tile_sched; /* device; layout documented at pf_attn_build_schedule */
   int32_t sched_stride;      /* int32 entries per (batch, q_tile) row */
-  int32_t variant;           /* 0 = default; 0x20 = the three-q-tile kernel; 0x10 = the two-q-tile kernel; 1 / 2 / 3 = the one-tile
-                              * kernel (A/B, see pf_attn.cu) */
+  int32_t variant;           /* 0 = default.  0x10 / 0x20 additionally require the pair / group schedule below; 1 / 2 / 3 are
+                              * accepted.  Every value runs the same kernel (pf_attn.cu) and gives the same bits. */
   int32_t q_row_begin;       /* only q rows >= q_row_begin are computed (multiple of 128; 0 = all).  The last single block
                               * needs the current clip's rows only (history outputs are discarded, reference F:380). */
-  const int32_t* pair_sched; /* device; built by pf_attn_build_pair_schedule from tile_sched, same sched_stride.  When set (and
-                              * variant does not ask for the one-tile kernel) the launch uses the two-q-tiles-per-CTA kernel. */
+  const int32_t* pair_sched; /* device; built by pf_attn_build_pair_schedule from tile_sched, same sched_stride.  Part of a
+                              * caller's plan; the kernel works from tile_sched and reads none of the pair / group arrays. */
   const int32_t* pair_mask_index; /* device; from pf_attn_build_pair_masks (required with pair_sched) */
   const void* pair_mask_bits;     /* device; [blocks, 128, 4] uint32 */
-  /* sequence parallelism (peer_count > 1, batch 1, two-q-tile kernel): row q of this rank's head group is stored into rank
+  /* sequence parallelism (peer_count > 1, batch 1): row q of this rank's head group is stored into rank
    * (q / peer_chunk_rows)'s buffer peer_out[...] at row q % peer_chunk_rows, columns peer_col_begin + h*64 (row stride ldo);
    * `out` is ignored. */
   void* peer_out[PF_MAX_PEERS];
   int32_t peer_count, peer_chunk_rows, peer_col_begin;
-  /* three-q-tile kernel (variant 0x20, or variant 0 under PF_OPT_ATTN_TRIPLE_KERNEL, the default): schedule and row masks of groups of three
+  /* variant 0x20: schedule and row masks of groups of three
    * q tiles from pf_attn_build_group_schedule / pf_attn_build_group_masks (group = 3), same sched_stride */
   const int32_t* group_sched;
   const int32_t* group_mask_index;
@@ -204,14 +204,14 @@ PF_API int pf_attn_build_schedule(const int32_t* seg_host, const int32_t* time_h
  * element mask (a tile without bit0 is computed fully masked).  `out` holds batch * ceil(q_tiles/2) rows of sched_stride. */
 PF_API int pf_attn_build_pair_schedule(const int32_t* tile_sched_host, int32_t batch, int32_t seq, int32_t sched_stride,
                                        int32_t* out);
-/* Host helper: the element masks of the two-q-tile kernel.  For every (pair entry, tile X) whose flags say "partial" it
+/* Host helper: the element masks of a pair schedule.  For every (pair entry, tile X) whose flags say "partial" it
  * assigns a block index (mask_index[batch, n_pairs, 2 * sched_stride], entry e / tile X at [2 e + X], -1 otherwise) and, when
  * mask_bits != NULL, fills block = 128 rows x 4 uint32: bit i of word w of row r = q row r of the tile may attend kv column
  * 32 w + i of the kv tile.  Returns the number of blocks needed (call once with mask_bits = NULL to size the buffer). */
 PF_API int64_t pf_attn_build_pair_masks(const int32_t* seg_host, const int32_t* time_host, const int32_t* pair_sched_host,
                                         int32_t batch, int32_t seq, int32_t sched_stride, int32_t* mask_index,
                                         uint32_t* mask_bits, int64_t capacity_blocks);
-/* Host helpers of the three-q-tile kernel, the pair forms generalised to groups of `group` (2..4) q tiles counted from the end
+/* Host helpers: the pair forms generalised to groups of `group` (2..4) q tiles counted from the end
  * of the sequence.  Entry = (kv_tile << 8) | flags, 2 flag bits per tile X at bit 2 X (X = 0 the lowest tile of the group);
  * mask_index[batch, n_groups, group * sched_stride], entry e / tile X at [group e + X]; blocks as in the pair form.  With
  * pair_sched_host / pair_mask_index_host (the pair schedule of the same tile_sched) no bits are built: the indices point into
@@ -269,7 +269,7 @@ PF_API int pf_cfg_euler_step(const float* v2, float guidance, float dsigma, cons
 PF_API int pf_stage_hop(const void* x, int32_t x_is_f32, const float* z, void* out, int64_t planes, int32_t h, int32_t w,
                         float alpha, float beta, const float* chol16, void* stream);
 
-/* ------------------------------------------------------------------ causal 3-D convolution (VAE decode, tcgen05 + TMA)
+/* ------------------------------------------------------------------ causal 3-D convolution (VAE decode, wgmma + TMA)
  * Replaces CausalConv3d -> nn.Conv3d (C:46-146), kernel 3x3x3 or 1x1x1, stride 1, on channels-last bf16 activations.
  * x: [B, T + kt - 1, H, W, Cin]: the (kt-1) causal-padding frames are physically present in front (zeros for the first
  * chunk, the previous chunk's last input frames afterwards = the reference's feature cache C:126-143); spatial zero
@@ -296,9 +296,8 @@ typedef struct pf_conv3d_desc {
   int32_t stride_t, stride_h, stride_w; /* 0/1 = unit stride; 2 = the encoder's down-samplers (C:66-67: CausalDownsample2x
                                          * stride (1,2,2) R:322, CausalTemporalDownsample2x stride (2,1,1) R:486).  b,t,h,w
                                          * stay OUTPUT dims; x is [B, (t-1)*stride_t + kt, h*stride_h, w*stride_w, cin]. */
-  int32_t kernel_variant; /* 0 = auto; 1 = 1-CTA tiles (conv3d); 2 = 2-CTA pairs, one TMA box per tap (conv3d2);
-                           * 3 = 2-CTA pairs with kw-tap reuse (conv3d2w: needs 128-voxel rows, 3x3x3, unit stride).
-                           * Every kernel accumulates in the same K order: the choice never changes the bits. */
+  int32_t kernel_variant; /* 0 = auto; 1 = 128-wide filter tiles (cout % 128 == 0); 2 = 64-wide filter tiles.
+                           * Both accumulate in the same K order: the choice never changes the bits. */
 } pf_conv3d_desc;
 PF_API int pf_causal_conv3d(const pf_conv3d_desc* desc, void* stream);
 
@@ -324,38 +323,6 @@ PF_API int pf_pack_latent(const void* z, int32_t z_is_f32, int32_t b, int32_t c,
  * blended axis: b[o, y, i] = a[o, la - extent + y, i] * (1 - y/extent) + b[o, y, i] * (y/extent) for y < extent (in place). */
 PF_API int pf_blend_tiles(const float* a, float* b, int64_t outer, int32_t la, int32_t lb, int64_t inner, int32_t extent,
                           void* stream);
-
-/* ------------------------------------------------------------------ debug probe (used only by tests/tools)
- * One CTA, one 128 x N x K tcgen05.mma chain with host-chosen descriptor bits, so descriptor encodings can be
- * pinned on hardware without recompiling.  a: bf16 [128, K] (K-major) or staged to TMEM when a_from_tmem;
- * b: bf16, loaded by TMA as [rows_b, cols_b] boxes of 64 columns.  d: fp32 [128, N]. */
-typedef struct pf_umma_probe {
-  const void* a;
-  const void* b;
-  float* d;
-  int32_t n, k;
-  int32_t b_rows, b_cols;  /* global shape of b (row-major) */
-  int32_t b_box_rows;      /* TMA box rows for b (box cols fixed at 64 = 128 B) */
-  int32_t b_mn_major;      /* instruction-descriptor bit 16 */
-  uint32_t b_lbo, b_sbo;   /* bytes */
-  uint32_t b_k_step_bytes; /* descriptor start-address advance per UMMA_K=16 inside a 64-wide k block */
-  uint32_t b_kblock_bytes; /* descriptor start-address advance per 4 UMMA_K steps (one 64-wide k block) */
-  int32_t a_from_tmem;     /* 1: A is converted to packed bf16 pairs in TMEM (lane = row, 32-bit column = 2 k) */
-  int32_t a_rows;          /* rows of a staged in shared memory (0 = 128); the MMA reads rows [a_row_offset, +128) */
-  int32_t a_row_offset;    /* start-address advance of the A descriptor in 128-byte rows (inside the swizzle atom) */
-  int32_t a_base_offset;   /* value of the descriptor's base-offset field, bits [49,52) */
-} pf_umma_probe;
-PF_API int pf_debug_umma(const pf_umma_probe* p, void* stream);
-
-/* Debug timeline of the attention kernel: `device_buf` = 3 * 48 * 8 uint64 (clock64 stamps of one CTA: two softmax warps
- * and the MMA issuer, first 48 kv tiles), filled by pf_attn_fwd_masked launches with variant bit 1 (value 2) set.  While a
- * buffer is set, launches of the two-q-tile kernel use its timeline instantiation and fill 4 x 64 x 12 uint64 instead
- * (softmax thread 0 of q tile A / B and the two MMA issuers of CTA (0, 0, 0), first 64 kv tiles).
- * NULL disables.  Test/profiling aid only (tools/gpu_check.py attn_trace). */
-PF_API int pf_debug_attn_trace(void* device_buf);
-/* Per-CTA records of the same trace variant: `device_buf` = capacity x 8 uint64 (clock64 at CTA entry, at exit, number of
- * kv tiles, SM id), indexed by the linear block index.  NULL disables. */
-PF_API int pf_debug_attn_cta_trace(void* device_buf, int64_t capacity);
 
 #ifdef __cplusplus
 }

@@ -12,7 +12,7 @@ Parity status: PINNED against the unmodified reference imported through oracle/p
 
 The same code serves two numerics modes:
   * fp32 (default): the "truth" the CUDA path is compared with;
-  * under `torch.autocast(device, torch.bfloat16)`: reproduces the reference's own bf16 dtype policy (SURVEY A.7) because
+  * under `torch.autocast(device, torch.bfloat16)`: reproduces the reference's own bf16 dtype policy because
     it uses the same torch ops the reference uses (F.linear, F.layer_norm, F.scaled_dot_product_attention, ...).
 """
 from __future__ import annotations

@@ -1,9 +1,9 @@
-"""Dependency shim so the UNMODIFIED reference (/root/reference) imports in this container.
+"""Dependency shim so the UNMODIFIED reference imports without its optional dependencies.
 
-TEST INFRASTRUCTURE, used only by oracle/pin/*.py (run in the build container where /root/reference exists) to pin
+TEST INFRASTRUCTURE, used only by oracle/pin/*.py (run where a checkout of the reference is readable) to pin
 the oracle restatement and to generate tests/golden/*.  Nothing shipped or measured imports this.
 
-The image lacks diffusers / accelerate / timm / tensorboardX / IPython (SURVEY.md §8c).  The pieces of those packages
+The reference imports diffusers / accelerate / timm / tensorboardX / IPython, which need not be installed.  The pieces of those packages
 the reference touches at import time are stubbed; the four that carry arithmetic are restated from the diffusers 0.30
 semantics (requirements.txt:6 pins diffusers>=0.30.1):
   * diffusers.models.activations.GELU            -> F.gelu(Linear(x), approximate=...)         (call sites B:73-75, MB:57-59)
@@ -25,9 +25,12 @@ import torch.nn.functional as F
 
 import os as _os
 
-# /root/reference in the build container; on the GPU box the byte-for-byte copy staged by oracle/pin/stage_reference.py
-_STAGED = _os.path.join(_os.path.dirname(_os.path.dirname(_os.path.dirname(_os.path.abspath(__file__)))), "baseline", "_ref")
-REFERENCE_ROOT = "/root/reference" if _os.path.isdir("/root/reference") else _STAGED
+# the checkout of the original project where it is readable (see oracle/pin/stage_reference.py), else the byte-for-byte copy
+# that script staged under oracle/_ref
+_ROOT = _os.path.dirname(_os.path.dirname(_os.path.dirname(_os.path.abspath(__file__))))
+_STAGED = _os.path.join(_ROOT, "oracle", "_ref")
+_SOURCE = _os.environ.get("PYRAMID_FLOW_REFERENCE") or _os.path.join(_os.path.dirname(_ROOT), "reference")
+REFERENCE_ROOT = _SOURCE if _os.path.isdir(_os.path.join(_SOURCE, "pyramid_dit")) else _STAGED
 
 
 def reference_available() -> bool:
@@ -213,7 +216,7 @@ class Attention(nn.Module):
 
 
 def install() -> None:
-    """Register the stubs and put /root/reference on sys.path."""
+    """Register the stubs and put the reference on sys.path."""
     import transformers  # noqa: F401  (must be imported before a version-less `accelerate` stub exists)
 
     d = _mod("diffusers")

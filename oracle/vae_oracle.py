@@ -4,7 +4,7 @@ Restates `CausalVideoVAE.decode` (video_vae/modeling_causal_vae.py:376-395) for 
 a state-dict in the reference key layout:
   V = video_vae/modeling_causal_vae.py     D = .../modeling_enc_dec.py     K = .../modeling_block.py
   R = .../modeling_resnet.py               C = .../modeling_causal_conv.py
-plus the mid-block attention from diffusers 0.30 `Attention(_from_deprecated_attn_block=True)` (not in /root/reference;
+plus the mid-block attention from diffusers 0.30 `Attention(_from_deprecated_attn_block=True)` (not in the reference checkout;
 pinned version diffusers>=0.30.1, requirements.txt:6; call sites K:413-427, K:458).
 
 Temporal chunking with the 2-frame feature cache (C:126-143, V:346-374) is EXACT w.r.t. the un-chunked computation

@@ -1,7 +1,7 @@
 """ctypes binding of libpf_b200.so (the C-ABI declared in include/pf_b200.h).
 
 PyTorch is used only for device memory and streams: every call passes raw `data_ptr()`s and the current CUDA stream.
-There is no fallback: if the library is missing or the device is not sm_100, calls raise RuntimeError.
+There is no fallback: if the library is missing or the device is not sm_90, calls raise RuntimeError.
 """
 from __future__ import annotations
 
@@ -24,9 +24,6 @@ SYMBOLS = [
     "pf_ctx_create", "pf_ctx_destroy", "pf_ctx_record_begin", "pf_ctx_record_end", "pf_ctx_replay", "pf_dit_step_flux",
     "pf_dit_step_mmdit", "pf_vae_decode_chunk",
     "pf_peer_alloc", "pf_peer_free", "pf_peer_export", "pf_peer_open", "pf_peer_close", "pf_peer_barrier", "pf_peer_bcast",
-    "pf_debug_umma",
-    "pf_debug_attn_trace",
-    "pf_debug_attn_cta_trace",
 ]
 
 PF_OPT_GEMM_STAGED_RESID, PF_OPT_GEMM_WAVE_TILING, PF_OPT_ATTN_PAIR_KERNEL, PF_OPT_ATTN_TILE_PHASE, PF_OPT_ATTN_TRIPLE_KERNEL = range(5)
@@ -86,16 +83,6 @@ class ConvDesc(C.Structure):
     ]
 
 
-class UmmaProbe(C.Structure):
-    _fields_ = [
-        ("a", C.c_void_p), ("b", C.c_void_p), ("d", C.c_void_p),
-        ("n", C.c_int32), ("k", C.c_int32),
-        ("b_rows", C.c_int32), ("b_cols", C.c_int32), ("b_box_rows", C.c_int32), ("b_mn_major", C.c_int32),
-        ("b_lbo", C.c_uint32), ("b_sbo", C.c_uint32), ("b_k_step_bytes", C.c_uint32), ("b_kblock_bytes", C.c_uint32),
-        ("a_from_tmem", C.c_int32), ("a_rows", C.c_int32), ("a_row_offset", C.c_int32), ("a_base_offset", C.c_int32),
-    ]
-
-
 _lib = None
 _warm_devices = set()
 
@@ -115,11 +102,6 @@ def load() -> C.CDLL:
         raise RuntimeError(f"libpf_b200.so does not export: {missing}")
     lib.pf_last_error.restype = C.c_char_p
     lib.pf_launch_count.restype = C.c_int64
-    if int(os.environ.get("WORLD_SIZE", "1")) > 2:
-        # world = CFG(2) x SP(world / 2): with SP > 1 the attention launches carry peer stores and run the two-q-tile kernel (the
-        # three-q-tile kernel has only been validated on one GPU).  Keep the WHOLE process on that kernel, so the single-GPU
-        # reference a sharded step is compared with (bench.py `parity_vs_n1`, tools/sp_check.py) stays bit-identical to it.
-        lib.pf_set_option(PF_OPT_ATTN_TRIPLE_KERNEL, 0)
     lib.pf_gemm_bf16.argtypes = [C.POINTER(GemmDesc), C.c_void_p]
     lib.pf_attn_fwd_masked.argtypes = [C.POINTER(AttnDesc), C.c_void_p]
     lib.pf_attn_build_schedule.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
@@ -156,9 +138,6 @@ def load() -> C.CDLL:
     lib.pf_stage_hop.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_float,
                                  C.c_float, C.POINTER(C.c_float), C.c_void_p]
     lib.pf_blend_tiles.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_void_p]
-    lib.pf_debug_umma.argtypes = [C.POINTER(UmmaProbe), C.c_void_p]
-    lib.pf_debug_attn_trace.argtypes = [C.c_void_p]
-    lib.pf_debug_attn_cta_trace.argtypes = [C.c_void_p, C.c_int64]
     lib.pf_causal_conv3d.argtypes = [C.POINTER(ConvDesc), C.c_void_p]
     lib.pf_groupnorm_stats.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_float, C.c_void_p,
                                        C.c_void_p, C.c_int64, C.c_void_p]

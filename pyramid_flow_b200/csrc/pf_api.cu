@@ -246,7 +246,7 @@ int pf_warmup(void) {
 }
 
 const char* pf_last_error(void) { return pf::g_err; }
-int pf_version(void) { return 100; }
+int pf_version(void) { return 200; }
 int64_t pf_launch_count(void) { return pf::g_launches.load(); }
 
 int pf_device_check(void) {
@@ -264,8 +264,8 @@ int pf_device_check(void) {
     pf::set_error("cudaGetDeviceProperties: %s", cudaGetErrorString(e));
     return -1;
   }
-  if (prop.major != 10) {
-    pf::set_error("libpf_b200 is built for sm_100a only; device is sm_%d%d", prop.major, prop.minor);
+  if (prop.major != 9) {
+    pf::set_error("libpf_b200 is built for sm_90a only; device is sm_%d%d", prop.major, prop.minor);
     return -1;
   }
   if (pf::get_encode_fn() == nullptr) {

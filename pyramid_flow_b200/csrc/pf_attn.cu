@@ -1,4 +1,4 @@
-// pf_attn.cu — masked joint text+video attention forward on tcgen05 tensor cores (head_dim 64).
+// pf_attn.cu — masked joint text+video attention forward on Hopper warpgroup MMA (head_dim 64).
 //
 //   out[b, q, h, :] = softmax_kv( q.k * scale  | mask(q, kv) ) . v ,   mask = (seg_q == seg_kv) && (time_q >= time_kv)
 //
@@ -6,20 +6,12 @@
 // built at F:318-350).  The mask is never materialised: a host-built tile schedule (pf_attn_build_schedule) lists, per
 // 128-row q tile, only the 128-wide kv tiles that contain an allowed pair and flags the few that need an element mask.
 //
-// One CTA = one (batch, head, 128-row q tile); 320 threads; two CTAs are co-resident per SM so that one CTA's softmax
-// (MUFU-bound at head_dim 64) overlaps the other CTA's tensor-core work:
-//   warps 0-7  softmax: thread == (q row == TMEM lane, 64-column half).  The thread's 64 scores are read from TMEM once
-//              and stay in registers for the FMNMX3 max pass and the ex2 pass.  The reference max is one tile stale: the
-//              two halves publish their partial max of tile j in shared memory and read the partner's for tile j-1
-//              (ordered by the P-ready mbarrier), so there is no per-tile pair barrier and the exps of tile j never
-//              wait for P.V(j-1).  P is written back to TMEM as packed bf16; O is rescaled in TMEM only when the
-//              reference moved by > 2^8 (lazy rescale)
-//   warp 8     MMA issuer (one lane): S = Q.K^T (SS: both operands in smem, K-major), O += P.V (TS: P from TMEM,
-//              V from smem MN-major — V is consumed in its natural [kv, hd] layout, no transpose)
-//   warp 9     TMA producer (one lane): Q once, then K tiles through a 3-stage and V tiles through a 2-stage mbarrier ring
-// S(j+1) = Q.K(j+1)^T is issued as soon as softmax(j) has pulled S(j) into registers, so the tensor pipe works under the
-// softmax instead of after it.
-// TMEM map (256 columns): S fp32 [0,128) | O fp32 [128,192) | P bf16x2 [192,256).
+// One CTA = one (batch, head, 128-row q tile); 384 threads:
+//   warpgroup 0 (one lane)  TMA producer: Q once, then K and V tiles through 2-stage mbarrier rings
+//   warpgroups 1, 2         64 q rows each: S = Q.K^T (wgmma, both operands in smem, K-major) lands in registers, the online
+//                           softmax (exact running max, exp2) runs on the accumulator fragments, P is re-packed in registers as
+//                           the bf16 A operand and O += P.V is a wgmma with A from registers and V from smem MN-major -- V is
+//                           consumed in its natural [kv, hd] layout, no transpose.
 #include <algorithm>
 #include <vector>
 
@@ -31,14 +23,10 @@ namespace pf {
 constexpr int ATT_BM = 128;      // q rows per CTA
 constexpr int ATT_BN = 128;      // kv columns per tile
 constexpr int ATT_HD = 64;
-constexpr int ATT_KSTAGES = 3;   // K is consumed one tile ahead (S(j+1) is issued during softmax(j)): deeper ring
-constexpr int ATT_VSTAGES = 2;
-constexpr int ATT_SOFTMAX_WARPS = 8;   // 2 warps per TMEM lane quarter: each owns 64 of the 128 kv columns of a row
-constexpr int ATT_THREADS = (ATT_SOFTMAX_WARPS + 2) * 32;
+constexpr int ATT_STAGES = 2;
+constexpr int ATT_THREADS = 384;
 constexpr int ATT_TILE_BYTES = ATT_BN * ATT_HD * 2;  // 16 KB
-constexpr int ATT_SMEM_BYTES = (1 + ATT_KSTAGES + ATT_VSTAGES) * ATT_TILE_BYTES + 1024;
-constexpr uint32_t ATT_TMEM_COLS = 256;
-constexpr uint32_t TM_S = 0, TM_O = 128, TM_P = 192;
+constexpr int ATT_SMEM_BYTES = (1 + 2 * ATT_STAGES) * ATT_TILE_BYTES + 1024;
 
 struct AttnArgs {
   __nv_bfloat16* out;
@@ -49,116 +37,26 @@ struct AttnArgs {
   const int* time;
   const int* sched;
   int sched_stride;
+  // sequence parallel: output rows go straight into the owning rank's buffer (pf_b200.h)
+  __nv_bfloat16* peer_out[PF_MAX_PEERS];
+  int peer_count, peer_chunk_rows, peer_col_begin;
 };
 
-// Debug timeline (variant bit 1): clock64 stamps of ONE CTA (batch 0, head 0, middle q tile) for the first
-// ATT_TRACE_ITERS kv tiles: [role 0 = softmax warp 0, 1 = softmax warp 4, 2 = MMA issuer][iteration][5 stamps].
-constexpr int ATT_TRACE_ITERS = 48;
-constexpr int ATT_TRACE_SLOTS = 8;
-__device__ unsigned long long* g_attn_trace = nullptr;
-// Per-CTA records of the trace variant: [linear CTA index][4] = (clock64 at entry, clock64 at exit, kv tiles, SM id) --
-// to separate the fixed per-CTA cost from the per-tile cost (regression over all CTAs in tools/gpu_check.py).
-__device__ unsigned long long* g_attn_cta_trace = nullptr;
-__device__ long long g_attn_cta_trace_cap = 0;
-template <int TRACE>
-__device__ __forceinline__ void trace_stamp(unsigned long long* tr, int role, int j, int slot) {
-  if (TRACE) {
-    if (tr != nullptr && j < ATT_TRACE_ITERS) tr[(role * ATT_TRACE_ITERS + j) * ATT_TRACE_SLOTS + slot] = clock64();
-  }
-}
-
-__device__ __forceinline__ float ex2f(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
-__device__ __forceinline__ float max3f(float a, float b, float c) {
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
-}
-
-// the two warps that share a TMEM lane quarter (column halves 0/1 of the same 32 rows) meet on their own named barrier
-__device__ __forceinline__ void pair_bar_sync(int quarter) {
-  switch (quarter) {   // immediate barrier ids keep the CTA's barrier allocation at 5 instead of 16
-    case 0: asm volatile("bar.sync 1, 64;" ::: "memory"); break;
-    case 1: asm volatile("bar.sync 2, 64;" ::: "memory"); break;
-    case 2: asm volatile("bar.sync 3, 64;" ::: "memory"); break;
-    default: asm volatile("bar.sync 4, 64;" ::: "memory"); break;
-  }
-}
-
-// apply the element mask to 32 scores (bit i of `bits` = column i allowed)
-__device__ __forceinline__ void mask32(uint32_t (&v)[32], uint32_t bits) {
-#pragma unroll
-  for (int i = 0; i < 32; ++i)
-    if (!((bits >> i) & 1u)) v[i] = 0xff800000u;  // -inf
-}
-
-__device__ __forceinline__ float max32(const uint32_t (&v)[32]) {
-  float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;
-#pragma unroll
-  for (int i = 0; i < 32; i += 8) {
-    m0 = max3f(m0, __uint_as_float(v[i + 0]), __uint_as_float(v[i + 1]));
-    m1 = max3f(m1, __uint_as_float(v[i + 2]), __uint_as_float(v[i + 3]));
-    m2 = max3f(m2, __uint_as_float(v[i + 4]), __uint_as_float(v[i + 5]));
-    m3 = max3f(m3, __uint_as_float(v[i + 6]), __uint_as_float(v[i + 7]));
-  }
-  return fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-}
-
-// 2^x on the FMA/ALU pipes (no MUFU): round-to-nearest split x = n + f, f in [-0.5, 0.5], cubic for 2^f (rel. err 6e-4,
-// well under bf16's 4e-3), n added into the exponent field.  Used for a fraction of the elements to unload the XU pipe,
-// which bounds this kernel at head_dim 64 (the trick of FlashAttention-4 on Blackwell).
-__device__ __forceinline__ float ex2_poly(float x) {
-  x = fmaxf(x, -126.f);
-  const float t = x + 12582912.f;   // 1.5 * 2^23
-  const float f = x - (t - 12582912.f);
-  float p = fmaf(f, 0.0555041086648216f, 0.2402264923172690f);
-  p = fmaf(p, f, 0.6931471805599453f);
-  p = fmaf(p, f, 1.0f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
-}
-
-// p = exp2(s*c - m_ref) for 32 scores -> 16 packed bf16x2; accumulates the row sum into 4 independent chains.
-// POLY = 1: every 4th element takes the polynomial path (25 % of the exponentials off the XU pipe).
-template <int POLY>
-__device__ __forceinline__ void exp32(const uint32_t (&v)[32], uint32_t (&pk)[16], float c, float m_ref, float (&l)[4]) {
-#pragma unroll
-  for (int i = 0; i < 16; i += 2) {
-    // the reference max is one tile stale: clamp the argument so a tile that overshoots it by > 2^126 saturates instead of
-    // producing inf/NaN (the two-q-tile kernel in pf_attn2.cu has an exact max and needs no clamp)
-    const float p0 = ex2f(fminf(fmaf(__uint_as_float(v[2 * i + 0]), c, -m_ref), 126.f));
-    const float p1 = ex2f(fminf(fmaf(__uint_as_float(v[2 * i + 1]), c, -m_ref), 126.f));
-    const float p2 = ex2f(fminf(fmaf(__uint_as_float(v[2 * i + 2]), c, -m_ref), 126.f));
-    const float x3 = fminf(fmaf(__uint_as_float(v[2 * i + 3]), c, -m_ref), 126.f);
-    const float p3 = POLY ? ex2_poly(x3) : ex2f(x3);
-    l[0] += p0; l[1] += p1; l[2] += p2; l[3] += p3;
-    pk[i] = pack_bf16x2(p0, p1);
-    pk[i + 1] = pack_bf16x2(p2, p3);
-  }
-}
-
-template <int POLY, int TRACE>
-__global__ void __launch_bounds__(ATT_THREADS, 2)
+__global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                 const __grid_constant__ CUtensorMap tm_v, const AttnArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_q = smem;
   uint8_t* smem_k = smem + ATT_TILE_BYTES;
-  uint8_t* smem_v = smem_k + ATT_KSTAGES * ATT_TILE_BYTES;
+  uint8_t* smem_v = smem_k + ATT_STAGES * ATT_TILE_BYTES;
 
-  __shared__ __align__(8) uint64_t bar_q, bar_s_full, bar_s_free, bar_p_full, bar_pv_done;
-  __shared__ __align__(8) uint64_t k_full[ATT_KSTAGES], k_empty[ATT_KSTAGES], v_full[ATT_VSTAGES], v_empty[ATT_VSTAGES];
-  __shared__ uint32_t tmem_slot;
-  __shared__ float xch[2][2][ATT_BM];  // [tile parity][column half][row]: partial row max published to the paired warp
-  __shared__ float lxch[2][ATT_BM];    // [column half][row]: partial row sums (epilogue)
-  __shared__ unsigned long long cta_stamp[4];   // trace variant: after alloc+sync, first S seen, softmax loop end, last PV issued
+  __shared__ __align__(8) uint64_t bar_q;
+  __shared__ __align__(8) uint64_t k_full[ATT_STAGES], k_empty[ATT_STAGES], v_full[ATT_STAGES], v_empty[ATT_STAGES];
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wgroup = warp >> 2;
   // heavy (late) q tiles first: they own the longest kv lists
   const int qt = a.q_tiles - 1 - static_cast<int>(blockIdx.x);
   const int h = blockIdx.y;
@@ -166,350 +64,198 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const int bh = b * a.heads + h;
   const int* sched = a.sched + (static_cast<size_t>(b) * a.q_tiles + qt) * a.sched_stride;
   const int n_kv = sched[0];
-  unsigned long long cta_t0 = 0;
-  if (TRACE) cta_t0 = clock64();
-  unsigned long long* tr_cta = nullptr;   // trace buffer if this CTA is the traced one
-  if (TRACE) {
-    if (b == 0 && h == 0 && qt == a.q_tiles / 2) tr_cta = g_attn_trace;
-  }
-  constexpr int W_MMA = ATT_SOFTMAX_WARPS, W_TMA = ATT_SOFTMAX_WARPS + 1;
 
-  if (warp == W_TMA && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_q);
     tma_prefetch_desc(&tm_k);
     tma_prefetch_desc(&tm_v);
-  }
-  if (warp == W_MMA && lane == 0) {
     mbar_init(&bar_q, 1);
-    mbar_init(&bar_s_full, 1);
-    mbar_init(&bar_s_free, ATT_SOFTMAX_WARPS * 32);
-    mbar_init(&bar_p_full, ATT_SOFTMAX_WARPS * 32);
-    mbar_init(&bar_pv_done, 1);
-    for (int i = 0; i < ATT_KSTAGES; ++i) {
+    for (int i = 0; i < ATT_STAGES; ++i) {
       mbar_init(&k_full[i], 1);
-      mbar_init(&k_empty[i], 1);
-    }
-    for (int i = 0; i < ATT_VSTAGES; ++i) {
+      mbar_init(&k_empty[i], 8);   // one arrival per consumer warp
       mbar_init(&v_full[i], 1);
-      mbar_init(&v_empty[i], 1);
+      mbar_init(&v_empty[i], 8);
     }
     fence_barrier_init();
   }
-  if (warp == 0) {
-    tmem_alloc(&tmem_slot, ATT_TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
-  if (TRACE) {
-    if (threadIdx.x == 0) cta_stamp[0] = clock64();
-  }
 
-  if (warp == W_TMA) {
-    if (elect_one()) {
+  if (wgroup == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
       // ===== TMA producer =====
       mbar_arrive_expect_tx(&bar_q, ATT_TILE_BYTES);
       tma_load_3d(smem_q, &tm_q, &bar_q, 0, qt * ATT_BM, bh);
-      int ks = 0, vs = 0;
-      uint32_t kph = 0, vph = 0;
+      int st = 0;
+      uint32_t ph = 0;
       for (int j = 0; j < n_kv; ++j) {
         const int kt = sched[1 + j] >> 1;
-        mbar_wait(&k_empty[ks], kph ^ 1);
-        mbar_arrive_expect_tx(&k_full[ks], ATT_TILE_BYTES);
-        tma_load_3d(smem_k + ks * ATT_TILE_BYTES, &tm_k, &k_full[ks], 0, kt * ATT_BN, bh);
-        mbar_wait(&v_empty[vs], vph ^ 1);
-        mbar_arrive_expect_tx(&v_full[vs], ATT_TILE_BYTES);
-        tma_load_3d(smem_v + vs * ATT_TILE_BYTES, &tm_v, &v_full[vs], 0, kt * ATT_BN, bh);
-        if (++ks == ATT_KSTAGES) {
-          ks = 0;
-          kph ^= 1;
-        }
-        if (++vs == ATT_VSTAGES) {
-          vs = 0;
-          vph ^= 1;
+        mbar_wait(&k_empty[st], ph ^ 1);
+        mbar_arrive_expect_tx(&k_full[st], ATT_TILE_BYTES);
+        tma_load_3d(smem_k + st * ATT_TILE_BYTES, &tm_k, &k_full[st], 0, kt * ATT_BN, bh);
+        mbar_wait(&v_empty[st], ph ^ 1);
+        mbar_arrive_expect_tx(&v_full[st], ATT_TILE_BYTES);
+        tma_load_3d(smem_v + st * ATT_TILE_BYTES, &tm_v, &v_full[st], 0, kt * ATT_BN, bh);
+        if (++st == ATT_STAGES) {
+          st = 0;
+          ph ^= 1;
         }
       }
     }
-  } else if (warp == W_MMA) {
-    if (elect_one()) {
-      // ===== MMA issuer =====
-      constexpr uint32_t idesc_qk = make_idesc_bf16(ATT_BM, ATT_BN, 0, 0);  // A = Q (K-major), B = K (K-major)
-      constexpr uint32_t idesc_pv = make_idesc_bf16(ATT_BM, ATT_HD, 0, 1);  // A = P (TMEM),    B = V (MN-major)
-      mbar_wait(&bar_q, 0);
-      const uint64_t dq = make_smem_desc_kmajor_sw128(smem_u32(smem_q));
-      // S(j+1) = Q.K(j+1)^T is issued as soon as the softmax warps have pulled S(j) into registers (bar_s_free), i.e.
-      // it runs on the tensor pipe while softmax(j) is still computing; O += P(j).V(j) follows when P(j) arrives.
-      int ks = 0, vs = 0;          // ring positions of the NEXT K tile to multiply and the CURRENT V tile
-      uint32_t kph = 0, vph = 0;
-      auto issue_qk = [&]() {
-        mbar_wait(&k_full[ks], kph);
-        tc_fence_after();
-        const uint64_t dk = make_smem_desc_kmajor_sw128(smem_u32(smem_k + ks * ATT_TILE_BYTES));
+    return;
+  }
+
+  // ===== consumers: thread (warp w of the warpgroup, g = lane / 4, t = lane % 4) holds rows r0 = 16 w + g and r0 + 8 of its
+  // warpgroup's 64 q rows, columns 8 i + 2 t, 8 i + 2 t + 1 of every 8-column group i (the wgmma accumulator fragment) =====
+  setmaxnreg_inc<232>();
+  const int wg = wgroup - 1;
+  const int g4 = lane >> 2, t4 = lane & 3;
+  const int row0 = wg * 64 + (warp & 3) * 16 + g4;
+  const float c = a.scale_log2;
+  const int* sg = a.seg + static_cast<size_t>(b) * a.seq;
+  const int* tm = a.time + static_cast<size_t>(b) * a.seq;
+  int seg_q[2], time_q[2];
 #pragma unroll
-        for (int kk = 0; kk < ATT_HD / 16; ++kk)
-          umma_ss(tmem_base + TM_S, dq + 2 * kk, dk + 2 * kk, idesc_qk, kk != 0);
-        umma_commit(&k_empty[ks]);
-        umma_commit(&bar_s_full);
-        if (++ks == ATT_KSTAGES) {
-          ks = 0;
-          kph ^= 1;
-        }
-      };
-      issue_qk();
-      for (int j = 0; j < n_kv; ++j) {
-        if (j + 1 < n_kv) {
-          mbar_wait(&bar_s_free, j & 1);          // S(j) is in registers
-          trace_stamp<TRACE>(tr_cta, 2, j, 0);
-          issue_qk();
-          trace_stamp<TRACE>(tr_cta, 2, j, 1);
-        }
-        mbar_wait(&bar_p_full, j & 1);
-        trace_stamp<TRACE>(tr_cta, 2, j, 2);
-        mbar_wait(&v_full[vs], vph);
-        tc_fence_after();
-        trace_stamp<TRACE>(tr_cta, 2, j, 3);
-        // V tile [128 kv x 64 hd], 128-byte rows: MN-major, 8-row k groups 1024 B apart, 16 kv rows (2048 B) per MMA
-        const uint32_t sv = smem_u32(smem_v + vs * ATT_TILE_BYTES);
-#pragma unroll
-        for (int kk = 0; kk < ATT_BN / 16; ++kk) {
-          const uint64_t dv = make_smem_desc(sv + kk * 2048, ATT_BN * 128, 1024);
-          umma_ts(tmem_base + TM_O, tmem_base + TM_P + kk * 8, dv, idesc_pv, (j | kk) != 0);
-        }
-        umma_commit(&v_empty[vs]);
-        umma_commit(&bar_pv_done);
-        trace_stamp<TRACE>(tr_cta, 2, j, 4);
-        if (TRACE) {
-          if (j == n_kv - 1) cta_stamp[3] = clock64();
-        }
-        if (++vs == ATT_VSTAGES) {
-          vs = 0;
-          vph ^= 1;
-        }
-      }
-    }
-  } else {
-    // ===== softmax + correction + epilogue (8 warps; thread = (row, column half)) =====
-    const int quarter = warp & 3;
-    const int half = warp >> 2;
-    const int row = quarter * 32 + lane;
-    const int qpos = qt * ATT_BM + row;
+  for (int r = 0; r < 2; ++r) {
+    const int qpos = qt * ATT_BM + row0 + 8 * r;
     const bool q_valid = qpos < a.seq;
-    const int seg_q = q_valid ? a.seg[static_cast<size_t>(b) * a.seq + qpos] : -0x7fffffff;
-    const int time_q = q_valid ? a.time[static_cast<size_t>(b) * a.seq + qpos] : -0x7fffffff;
-    const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t t_s = tmem_base + lane_base + TM_S + half * 64;
-    const uint32_t t_o = tmem_base + lane_base + TM_O + half * 32;
-    const uint32_t t_p = tmem_base + lane_base + TM_P + half * 32;
-    const float c = a.scale_log2;
-    // Reference max of the row (raw score units), identical in both column halves.  It is STALE by one tile: tile j is
-    // exponentiated against the max over tiles < j (tile 0: exact, one paired exchange), and the max of tile j-1 -- each
-    // half publishes its partial in `xch`, ordered by bar_p_full(j-1) -- only raises the reference for tile j when it
-    // grew by more than 2^8 (lazy rescale).  bf16 P and the fp32 accumulators have fp32's exponent range, so a tile that
-    // overshoots the stale reference is exact as long as scores do not jump by > ~2^100 between neighbouring tiles
-    // (logits of RMS-normed q/k are bounded far below that).  This removes the per-tile pair barrier and the wait on
-    // P.V(j-1) from the softmax critical path: exps need only registers; P.V(j-1) is awaited just before P is stored.
-    float m_run = -INFINITY;        // -inf: no finite score seen yet, reference 0
-    float m_prev_part = -INFINITY;  // this half's partial max of the previous tile
-    float l4[4] = {0.f, 0.f, 0.f, 0.f};  // this half's partial row sum (4 chains)
-    unsigned long long* tr_me = (lane == 0 && quarter == 0) ? tr_cta : nullptr;
-    int entry = sched[1];
-
-    for (int j = 0; j < n_kv; ++j) {
-      const int kt = entry >> 1;
-      const bool masked = (entry & 1) != 0;
-      if (j + 1 < n_kv) entry = __ldg(sched + 2 + j);   // next tile's entry: its latency hides under this iteration
-      uint32_t allow0 = 0xffffffffu, allow1 = 0xffffffffu;
-      if (masked) {
-        const int* sg = a.seg + static_cast<size_t>(b) * a.seq;
-        const int* tm = a.time + static_cast<size_t>(b) * a.seq;
-        uint32_t bits0 = 0, bits1 = 0;
-        for (int i = 0; i < 32; ++i) {
-          const int kv0 = kt * ATT_BN + half * 64 + i;
-          const int kv1 = kv0 + 32;
-          bool ok0 = false, ok1 = false;
-          if (kv0 < a.seq) ok0 = (__ldg(sg + kv0) == seg_q) && (__ldg(tm + kv0) <= time_q);
-          if (kv1 < a.seq) ok1 = (__ldg(sg + kv1) == seg_q) && (__ldg(tm + kv1) <= time_q);
-          bits0 |= (ok0 ? 1u : 0u) << i;
-          bits1 |= (ok1 ? 1u : 0u) << i;
-        }
-        allow0 = bits0;
-        allow1 = bits1;
-      }
-      // The three waits of an iteration (P-ready of tile j-1, S(j), P.V(j-1)) are probed early and consumed late: every
-      // mbarrier / shared-memory round trip queues behind the other CTA's MUFU stream in the MIO queue (~300 cycles),
-      // so they are overlapped with each other and with the exps instead of being paid one after the other.
-      bool pf_ok = true;
-      if (j > 0) pf_ok = mbar_test(&bar_p_full, (j - 1) & 1);
-      const bool s_ok = mbar_test(&bar_s_full, j & 1);
-      float m_partner = -INFINITY;
-      if (j > 0) {
-        if (!pf_ok) mbar_wait(&bar_p_full, (j - 1) & 1);   // every softmax thread finished tile j-1: partials published
-        m_partner = xch[(j - 1) & 1][half ^ 1][row];
-      }
-      if (!s_ok) mbar_wait(&bar_s_full, j & 1);
-      tc_fence_after();
-      trace_stamp<TRACE>(tr_me, half, j, 0);
-      if (TRACE) {
-        if (j == 0 && threadIdx.x == 0) cta_stamp[1] = clock64();
-      }
-
-      // ---- this thread's 64 scores stay in registers for both the max and the exp
-      uint32_t va[32], vb[32];
-      tmem_ld32(t_s, va);
-      tmem_ld32(t_s + 32, vb);
-      tmem_ld_wait();
-      trace_stamp<TRACE>(tr_me, half, j, 1);
-      tc_fence_before();
-      mbar_arrive(&bar_s_free);   // S(j) now lives in registers: the tensor pipe may overwrite it with S(j+1)
-      if (masked) {
-        mask32(va, allow0);
-        mask32(vb, allow1);
-      }
-      const float m_part = fmaxf(max32(va), max32(vb));
-      if (TRACE) {   // keep the stamp behind the max (it would otherwise float above the FMNMX chain)
-        if (m_part == 12345.678f) trace_stamp<TRACE>(tr_me, half, j, 7);
-      }
-      trace_stamp<TRACE>(tr_me, half, j, 5);
-      float m_tile;   // exact max (both halves) of the newest tile that is known: tile 0 at j == 0, else tile j-1
-      if (j == 0) {
-        xch[0][half][row] = m_part;
-        pair_bar_sync(quarter);
-        m_tile = fmaxf(m_part, xch[0][half ^ 1][row]);
-      } else {
-        m_tile = fmaxf(m_prev_part, m_partner);
-        xch[j & 1][half][row] = m_part;   // slot (j & 1) was last read by the partner before its P-ready arrive of tile j-1
-      }
-      m_prev_part = m_part;
-      trace_stamp<TRACE>(tr_me, half, j, 2);
-
-      // ---- lazy rescale decision (per row, same in both halves)
-      const float m_cand = fmaxf(m_run, m_tile);
-      float alpha = 1.f;
-      bool need = false;
-      if (m_cand > m_run) {
-        if (m_run == -INFINITY || (m_cand - m_run) * c > 8.f) {
-          const float ref_old = (m_run == -INFINITY) ? 0.f : m_run * c;
-          if (j > 0) {
-            need = true;
-            alpha = ex2f(fminf(fmaxf(ref_old - m_cand * c, -126.f), 126.f));
-          }
-          m_run = m_cand;
-        }
-      }
+    seg_q[r] = q_valid ? sg[qpos] : -0x7fffffff;
+    time_q[r] = q_valid ? tm[qpos] : -0x7fffffff;
+  }
+  float m_run[2] = {-INFINITY, -INFINITY};   // running row max (raw score units); -inf: no allowed score seen yet
+  float l_run[2] = {0.f, 0.f};               // this thread's part of the row sum (its 32 of every tile's 128 columns)
+  float o[32];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) l4[i] *= alpha;
-      const float m_ref = (m_run == -INFINITY) ? 0.f : m_run * c;
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
 
-      // ---- p = exp2(s*c - m_ref), packed bf16x2, still in registers
-      bool pv_ok = true;
-      if (j > 0) pv_ok = mbar_test(&bar_pv_done, (j - 1) & 1);   // probe now, consume after the exps
-      uint32_t pk0[16], pk1[16];
-      if (POLY && !masked) {
-        exp32<1>(va, pk0, c, m_ref, l4);
-        exp32<1>(vb, pk1, c, m_ref, l4);
-      } else {
-        exp32<0>(va, pk0, c, m_ref, l4);
-        exp32<0>(vb, pk1, c, m_ref, l4);
-      }
-      trace_stamp<TRACE>(tr_me, half, j, 3);
+  mbar_wait(&bar_q, 0);
+  const uint64_t dq = make_smem_desc_kmajor_sw128(smem_u32(smem_q) + wg * (64 * 128));
+  int st = 0;
+  uint32_t ph = 0;
+  for (int j = 0; j < n_kv; ++j) {
+    const int entry = sched[1 + j];
+    const int kt = entry >> 1;
+    const bool masked = (entry & 1) != 0;
 
-      // ---- P(j-1) must have been consumed and O(j-1) produced by P.V(j-1) before P is overwritten / O is rescaled
-      if (j > 0) {
-        if (!pv_ok) mbar_wait(&bar_pv_done, (j - 1) & 1);
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, need)) {
-#pragma unroll 1
-          for (int cc = 0; cc < 32; cc += 16) {
-            uint32_t o[16];
-            tmem_ld16(t_o + cc, o);
-            tmem_ld_wait();
+    // ---- S = Q.K^T
+    float s[64];
+    mbar_wait(&k_full[st], ph);
+    {
+      const uint64_t dk = make_smem_desc_kmajor_sw128(smem_u32(smem_k + st * ATT_TILE_BYTES));
+      wgmma_fence();
 #pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st16(t_o + cc, o);
+      for (int kk = 0; kk < ATT_HD / 16; ++kk) wgmma_ss_n128(s, dq + 2 * kk, dk + 2 * kk, kk != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_reg_fence(s);
+    }
+    if (lane == 0) mbar_arrive(&k_empty[st]);
+
+    if (masked) {
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int kv = kt * ATT_BN + 8 * i + 2 * t4 + e;
+          int sk = 0x7fffffff, tk = 0x7fffffff;   // outside the sequence: matches no row
+          if (kv < a.seq) {
+            sk = __ldg(sg + kv);
+            tk = __ldg(tm + kv);
           }
+          if (!(sk == seg_q[0] && tk <= time_q[0])) s[4 * i + e] = -INFINITY;
+          if (!(sk == seg_q[1] && tk <= time_q[1])) s[4 * i + 2 + e] = -INFINITY;
         }
       }
-      tmem_st16(t_p, pk0);
-      tmem_st16(t_p + 16, pk1);
-      tmem_st_wait();
-      trace_stamp<TRACE>(tr_me, half, j, 4);
-      tc_fence_before();
-      mbar_arrive(&bar_p_full);
-      trace_stamp<TRACE>(tr_me, half, j, 6);
     }
 
-    if (TRACE) {
-      if (threadIdx.x == 0) cta_stamp[2] = clock64();
-    }
-    // ---- epilogue: combine the two halves' row sums, O / l -> bf16 -> out[b, qpos, h*64 + half*32 .. +32]
-    const float l_part = (l4[0] + l4[1]) + (l4[2] + l4[3]);
-    lxch[half][row] = l_part;
-    pair_bar_sync(quarter);
-    const float l_run = l_part + lxch[half ^ 1][row];
-    mbar_wait(&bar_pv_done, (n_kv - 1) & 1);
-    tc_fence_after();
-    const float inv = (l_run > 0.f) ? 1.f / l_run : 0.f;
-    __nv_bfloat16* dst = a.out + (static_cast<size_t>(b) * a.seq + qpos) * a.ldo + h * ATT_HD + half * 32;
-    uint32_t o[32];
-    tmem_ld32(t_o, o);
-    tmem_ld_wait();
-    if (q_valid) {
-      uint4* d4 = reinterpret_cast<uint4*>(dst);
+    // ---- online softmax on the fragments: row max over the thread's columns, then over the 4 threads of the row
+    float alpha[2];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        uint4 u;
-        u.x = pack_bf16x2(__uint_as_float(o[8 * i + 0]) * inv, __uint_as_float(o[8 * i + 1]) * inv);
-        u.y = pack_bf16x2(__uint_as_float(o[8 * i + 2]) * inv, __uint_as_float(o[8 * i + 3]) * inv);
-        u.z = pack_bf16x2(__uint_as_float(o[8 * i + 4]) * inv, __uint_as_float(o[8 * i + 5]) * inv);
-        u.w = pack_bf16x2(__uint_as_float(o[8 * i + 6]) * inv, __uint_as_float(o[8 * i + 7]) * inv);
-        d4[i] = u;
+    for (int r = 0; r < 2; ++r) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < 16; ++i) mx = fmaxf(mx, fmaxf(s[4 * i + 2 * r], s[4 * i + 2 * r + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[r], mx);
+      // m_new == -inf: every score so far is masked, the reference is 0 and nothing is rescaled
+      alpha[r] = (m_new == -INFINITY) ? 1.f : ex2_approx_f((m_run[r] - m_new) * c);
+      m_run[r] = m_new;
+      const float m_ref = (m_new == -INFINITY) ? 0.f : m_new * c;
+      float sum = 0.f;
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const float p0 = ex2_approx_f(fmaf(s[4 * i + 2 * r], c, -m_ref));
+        const float p1 = ex2_approx_f(fmaf(s[4 * i + 2 * r + 1], c, -m_ref));
+        s[4 * i + 2 * r] = p0;
+        s[4 * i + 2 * r + 1] = p1;
+        sum += p0 + p1;
       }
+      l_run[r] = l_run[r] * alpha[r] + sum;
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      o[4 * i + 0] *= alpha[0];
+      o[4 * i + 1] *= alpha[0];
+      o[4 * i + 2] *= alpha[1];
+      o[4 * i + 3] *= alpha[1];
+    }
+
+    // ---- O += P.V: the S fragment of columns [16 kk, 16 kk + 16) is exactly the A fragment of k step kk
+    mbar_wait(&v_full[st], ph);
+    {
+      const uint32_t sv = smem_u32(smem_v + st * ATT_TILE_BYTES);
+      uint32_t pa[ATT_BN / 16][4];   // all eight A fragments are packed before the fence: the MMA chain is issued back to back
+#pragma unroll
+      for (int kk = 0; kk < ATT_BN / 16; ++kk) {
+        pa[kk][0] = pack_bf16x2(s[8 * kk + 0], s[8 * kk + 1]);
+        pa[kk][1] = pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]);
+        pa[kk][2] = pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]);
+        pa[kk][3] = pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7]);
+      }
+      wgmma_reg_fence(o);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < ATT_BN / 16; ++kk) {
+        // V tile [128 kv x 64 hd], 128-byte rows: MN-major, 8-row k groups 1024 B apart, 16 kv rows (2048 B) per MMA
+        const uint64_t dv = make_smem_desc(sv + kk * 2048, ATT_BN * 128, 1024);
+        wgmma_rs_n64_tb(o, pa[kk], dv);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_reg_fence(o);
+    }
+    if (lane == 0) mbar_arrive(&v_empty[st]);
+    if (++st == ATT_STAGES) {
+      st = 0;
+      ph ^= 1;
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, ATT_TMEM_COLS);
-  }
-  if (TRACE) {
-    if (threadIdx.x == 0 && g_attn_cta_trace != nullptr) {
-      const long long idx = (static_cast<long long>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
-      if (idx < g_attn_cta_trace_cap) {
-        unsigned smid;
-        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-        unsigned long long* r = g_attn_cta_trace + idx * 8;
-        r[0] = cta_t0;
-        r[1] = clock64();
-        r[2] = static_cast<unsigned long long>(n_kv);
-        r[3] = smid;
-        r[4] = cta_stamp[0];
-        r[5] = cta_stamp[1];
-        r[6] = cta_stamp[2];
-        r[7] = cta_stamp[3];
-      }
+  // ---- epilogue: O / l -> bf16 -> out[b, qpos, h*64 + ...]
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    float l = l_run[r];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = (l > 0.f) ? 1.f / l : 0.f;
+    const int qpos = qt * ATT_BM + row0 + 8 * r;
+    if (qpos >= a.seq) continue;
+    __nv_bfloat16* dst;
+    if (a.peer_count > 1) {
+      const int pr = qpos / a.peer_chunk_rows;
+      dst = a.peer_out[pr] + static_cast<size_t>(qpos - pr * a.peer_chunk_rows) * a.ldo + a.peer_col_begin + h * ATT_HD;
+    } else {
+      dst = a.out + (static_cast<size_t>(b) * a.seq + qpos) * a.ldo + h * ATT_HD;
     }
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      *reinterpret_cast<uint32_t*>(dst + 8 * i + 2 * t4) = pack_bf16x2(o[4 * i + 2 * r] * inv, o[4 * i + 2 * r + 1] * inv);
   }
 }
 
-int warmup_attn2();
-void attn2_set_trace(unsigned long long* p, long long cap);
-void attn2_set_timeline(unsigned long long* p);
-
-int attn2_launch(const pf_attn_desc* d, cudaStream_t stream);
-int attn3q_launch(const pf_attn_desc* d, cudaStream_t stream);
-int warmup_attn3q();
-
 int warmup_attn() {
-  int rc = warmup_attn2();
-  if (!rc) rc = warmup_attn3q();
-ensure_dyn_smem(reinterpret_cast<const void*>(attn_fwd_kernel<0, 0>), ATT_SMEM_BYTES, "attn_fwd_kernel<0,0>");
-  if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_fwd_kernel<1, 0>), ATT_SMEM_BYTES, "attn_fwd_kernel<1,0>");
-  if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_fwd_kernel<0, 1>), ATT_SMEM_BYTES, "attn_fwd_kernel<0,1>");
-  return rc;
+  return ensure_dyn_smem(reinterpret_cast<const void*>(attn_fwd_kernel), ATT_SMEM_BYTES, "attn_fwd_kernel");
 }
 
 }  // namespace pf
@@ -579,25 +325,21 @@ extern "C" int pf_attn_fwd_masked(const pf_attn_desc* d, void* stream_) {
   PF_REQUIRE(d->q_row_begin >= 0 && d->q_row_begin % ATT_BM == 0 && d->q_row_begin < d->seq,
              "pf_attn_fwd_masked: q_row_begin %d must be a multiple of %d inside the sequence", d->q_row_begin, ATT_BM);
   PF_REQUIRE(d->ldo % 8 == 0 && (reinterpret_cast<uintptr_t>(d->out) & 15) == 0, "pf_attn_fwd_masked: out must be 16-byte aligned");
-  PF_REQUIRE(d->peer_count <= 1 || d->pair_sched != nullptr, "pf_attn_fwd_masked: peer stores need the two-q-tile kernel (pair_sched)");
-
-  // variant: 0 = default (the three-q-tile kernel pf_attn3q.cu when its group schedule is given and the launch has no peer stores,
-  // else the two-q-tile kernel pf_attn2.cu when a pair schedule is given, else the one-tile kernel below);
-  // 0x10 = the two-q-tile kernel, explicitly; 1 / 2 / 3 = the one-tile kernel (polynomial mix / clock trace / plain), kept for A/B
+  // Every variant value runs the one kernel of this file; the values that name a q-tile grouping still require the schedule
+  // they were defined with, so a caller's plan stays checked.
   PF_REQUIRE(d->variant == 0x10 || d->variant == 0x20 || (d->variant >= 0 && d->variant <= 3), "pf_attn_fwd_masked: bad variant 0x%x", d->variant);
-  // 0x20 = the three-q-tile kernel (pf_attn3q.cu), also variant 0 under PF_OPT_ATTN_TRIPLE_KERNEL when its schedule is given
-  if (d->variant == 0x20 ||
-      (d->variant == 0 && d->group_sched != nullptr && d->peer_count <= 1 && get_option(PF_OPT_ATTN_TRIPLE_KERNEL))) {
+  if (d->variant == 0x20)
     PF_REQUIRE(d->group_sched != nullptr && d->group_mask_index != nullptr && d->group_mask_bits != nullptr,
                "pf_attn_fwd_masked: variant 0x%x needs group_sched, group_mask_index and group_mask_bits", d->variant);
-    return attn3q_launch(d, stream);
-  }
-  const bool use_pair = d->variant == 0x10 || (d->variant == 0 && d->pair_sched != nullptr && (get_option(PF_OPT_ATTN_PAIR_KERNEL) || d->peer_count > 1));
-  PF_REQUIRE(d->peer_count <= 1 || use_pair, "pf_attn_fwd_masked: peer stores are implemented by the two-q-tile kernel only");
-  if (use_pair) {
+  if (d->variant == 0x10)
     PF_REQUIRE(d->pair_sched != nullptr && d->pair_mask_index != nullptr && d->pair_mask_bits != nullptr,
                "pf_attn_fwd_masked: variant 0x%x needs pair_sched, pair_mask_index and pair_mask_bits", d->variant);
-    return attn2_launch(d, stream);
+  if (d->peer_count > 1) {
+    PF_REQUIRE(d->batch == 1 && d->peer_count <= PF_MAX_PEERS && d->peer_chunk_rows > 0 &&
+                   static_cast<long long>(d->peer_chunk_rows) * d->peer_count >= d->seq && d->peer_col_begin % 8 == 0,
+               "pf_attn_fwd_masked: bad peer layout (batch %d, count %d, chunk rows %d, seq %d)", d->batch, d->peer_count,
+               d->peer_chunk_rows, d->seq);
+    for (int i = 0; i < d->peer_count; ++i) PF_REQUIRE(d->peer_out[i] != nullptr, "pf_attn_fwd_masked: peer_out[%d] is null", i);
   }
   CUtensorMap tm[3];
   const void* ptrs[3] = {d->q, d->k, d->v};
@@ -621,41 +363,14 @@ extern "C" int pf_attn_fwd_masked(const pf_attn_desc* d, void* stream_) {
   a.time = d->time;
   a.sched = d->tile_sched;
   a.sched_stride = d->sched_stride;
+  a.peer_count = d->peer_count;
+  a.peer_chunk_rows = d->peer_chunk_rows;
+  a.peer_col_begin = d->peer_col_begin;
+  for (int i = 0; i < PF_MAX_PEERS; ++i) a.peer_out[i] = static_cast<__nv_bfloat16*>(d->peer_out[i]);
 
   if (int rc = warmup_attn()) return rc;
   // q tile index = q_tiles - 1 - blockIdx.x: a shorter grid.x drops the leading (lowest) q tiles
   dim3 grid(q_tiles - d->q_row_begin / ATT_BM, d->heads, d->batch);
-  if (d->variant == 2)
-    attn_fwd_kernel<0, 1><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tm[0], tm[1], tm[2], a);
-  else if (d->variant == 1)
-    attn_fwd_kernel<1, 0><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tm[0], tm[1], tm[2], a);
-  else
-    attn_fwd_kernel<0, 0><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tm[0], tm[1], tm[2], a);
+  attn_fwd_kernel<<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tm[0], tm[1], tm[2], a);
   return check_launch("pf_attn_fwd_masked");
-}
-
-// Debug: per-CTA records (4 uint64 each, `capacity` CTAs) filled by the variant-2 (trace) kernel; NULL disables.
-extern "C" int pf_debug_attn_cta_trace(void* device_buf, int64_t capacity) {
-  unsigned long long* p = static_cast<unsigned long long*>(device_buf);
-  long long cap = device_buf ? capacity : 0;
-  pf::attn2_set_trace(p, cap);
-  cudaError_t e = cudaMemcpyToSymbol(pf::g_attn_cta_trace, &p, sizeof(p));
-  if (e == cudaSuccess) e = cudaMemcpyToSymbol(pf::g_attn_cta_trace_cap, &cap, sizeof(cap));
-  if (e != cudaSuccess) {
-    pf::set_error("pf_debug_attn_cta_trace: %s", cudaGetErrorString(e));
-    return -2;
-  }
-  return 0;
-}
-
-// Debug: device buffer of 3 * 48 * 8 uint64 clock stamps filled by the variant-2 (trace) kernel; NULL disables.
-extern "C" int pf_debug_attn_trace(void* device_buf) {
-  unsigned long long* p = static_cast<unsigned long long*>(device_buf);
-  pf::attn2_set_timeline(p);   // the E/C-phase kernel's timeline instantiation: 4 roles x 64 iterations x 12 slots
-  cudaError_t e = cudaMemcpyToSymbol(pf::g_attn_trace, &p, sizeof(p));
-  if (e != cudaSuccess) {
-    pf::set_error("pf_debug_attn_trace: %s", cudaGetErrorString(e));
-    return -2;
-  }
-  return 0;
 }

@@ -1,14 +1,14 @@
-// pf_conv.cu — causal 3-D convolution (k = 3x3x3 or 1x1x1, stride 1) as an im2col-free implicit GEMM on tcgen05.
+// pf_conv.cu — causal 3-D convolution (k = 3x3x3 or 1x1x1, stride 1) as an im2col-free implicit GEMM on Hopper wgmma.
 //
 // Replaces CausalConv3d -> nn.Conv3d (reference video_vae/modeling_causal_conv.py:116-146, cuDNN conv3d on NCDHW) for
 // the VAE decoder.  Activations are channels-last bf16 [B, T, H, W, C]; an output tile is a TH x TW spatial patch of one
-// frame (128 voxels = the UMMA M), and the K loop walks (tap, 64-channel chunk):
+// frame (128 voxels = two 64-row wgmma slices), and the K loop walks (tap, 64-channel chunk):
 //   A tile  = ONE 5-D TMA box (64 ch, TW, TH, 1 frame, 1 batch) at the tap-shifted coordinate.  Out-of-bounds spatial
 //             coordinates are zero-filled by TMA => the conv's spatial zero padding costs nothing; the causal temporal
 //             padding is (kt-1) leading frames physically present in the input buffer (zeros for the first chunk, the
 //             previous chunk's last frames afterwards — the reference's feature cache, C:126-143).
 //   B tile  = weights re-laid out as [Cout, taps*Cin] (tap-major), a plain 2-D TMA box like the GEMM.
-// The box lands in shared memory as [TH][TW][64] = 128 rows of 128 B with SWIZZLE_128B, i.e. exactly the K-major UMMA
+// The box lands in shared memory as [TH][TW][64] = 128 rows of 128 B with SWIZZLE_128B, i.e. exactly the K-major wgmma
 // operand; no im2col buffer exists anywhere.  Pipeline / warp roles are the GEMM's (pf_gemm.cu).
 // Epilogue: bias (+ residual) -> bf16/fp32 channels-last store, optionally through the depth-to-space addressing of
 // CausalUpsample2x (R:616) / CausalTemporalUpsample2x (R:724-727) so the rearrange copy disappears.
@@ -23,7 +23,6 @@ struct ConvArgs {
   int b, t, h, w, cin;
   int cout;            // padded N actually computed (multiple of BN)
   int taps, kt, kh, kw;
-  int kw_baseoff;      // kw-reuse kernel: set the A descriptor's base-offset field to the row offset (debug switch)
   int st, sh, sw;      // conv stride (t, h, w): 1, or 2 for the encoder's down-samplers; (b, t, h, w) are OUTPUT dims
   int th, tw, tiles_h, tiles_w;
   int n_tiles;
@@ -37,34 +36,26 @@ struct ConvArgs {
   int res_t_total, res_t_offset;
 };
 
-constexpr int CBM = 128;
-constexpr int CBK = 64;
-constexpr int CONV_THREADS = 256;
+constexpr int CBK = PIPE_BK;
 
+// Epilogue of one staged accumulator row: this thread owns voxel (bb, tt, hh, ww) and every second 16-channel chunk
+// (starting at chunk `half`) of conv channels [n_base, n_base+BN); `srow` = the voxel's fp32 accumulators in shared memory.
 template <int BN>
-struct ConvCfg {
-  static constexpr int A_BYTES = CBM * CBK * 2;
-  static constexpr int B_BYTES = BN * CBK * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BN >= 256) ? 4 : (BN >= 128) ? 6 : 8;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;
-  static constexpr int TMEM_COLS = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-};
-
-// Epilogue of one 128-voxel accumulator slice: this thread owns voxel (bb, tt, hh, ww), conv channels [n_base, n_base+BN).
-template <int BN>
-__device__ __forceinline__ void conv_epilogue_tile(const ConvArgs& g, uint32_t taddr, int bb, int tt, int hh, int ww,
-                                                   bool valid, int n_base) {
+__device__ __forceinline__ void conv_epilogue_tile(const ConvArgs& g, const float* srow, int half, int bb, int tt, int hh,
+                                                   int ww, bool valid, int n_base) {
 #pragma unroll 1
-  for (int c = 0; c < BN / 16; ++c) {
-    uint32_t v[16];
-    tmem_ld16(taddr + c * 16, v);
-    tmem_ld_wait();
+  for (int c = half; c < BN / 16; c += 2) {
     const int n0 = n_base + c * 16;
     if (!valid || n0 >= g.store_channels) continue;
     float x[16];
 #pragma unroll
-    for (int i = 0; i < 16; ++i) x[i] = __uint_as_float(v[i]) + (g.bias ? __ldg(g.bias + n0 + i) : 0.f);
+    for (int i = 0; i < 4; ++i) {
+      const float4 v = *reinterpret_cast<const float4*>(srow + c * 16 + 4 * i);
+      x[4 * i + 0] = v.x + (g.bias ? __ldg(g.bias + n0 + 4 * i + 0) : 0.f);
+      x[4 * i + 1] = v.y + (g.bias ? __ldg(g.bias + n0 + 4 * i + 1) : 0.f);
+      x[4 * i + 2] = v.z + (g.bias ? __ldg(g.bias + n0 + 4 * i + 2) : 0.f);
+      x[4 * i + 3] = v.w + (g.bias ? __ldg(g.bias + n0 + 4 * i + 3) : 0.f);
+    }
     if (g.store_mode == 0) {
       const int to = tt + g.out_t_offset;
       if (to < 0 || to >= g.out_t_total) continue;
@@ -152,45 +143,30 @@ __device__ __forceinline__ void conv_epilogue_tile(const ConvArgs& g, uint32_t t
 }
 
 template <int BN>
-__global__ void __launch_bounds__(CONV_THREADS, 1)
-conv3d_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w, const ConvArgs g) {
-  using Cfg = ConvCfg<BN>;
+__global__ void __launch_bounds__(PIPE_THREADS, 1)
+conv3d_wgmma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w, const ConvArgs g) {
+  using Cfg = PipeCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  float* acc_tile = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
 
   __shared__ __align__(8) uint64_t full_bar[STAGES];
   __shared__ __align__(8) uint64_t empty_bar[STAGES];
-  __shared__ __align__(8) uint64_t tmem_full_bar[2];
-  __shared__ __align__(8) uint64_t tmem_empty_bar[2];
-  __shared__ uint32_t tmem_base_slot;
 
   const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wgroup = warp >> 2;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_x);
     tma_prefetch_desc(&tm_w);
-  }
-  if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full_bar[i], 1);
-      mbar_init(&tmem_empty_bar[i], 128);
+      mbar_init(&empty_bar[i], PIPE_CONSUMER_WARPS);
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(&tmem_base_slot, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_slot;
 
   const int cchunks = g.cin / CBK;
   const int num_kb = g.taps * cchunks;
@@ -198,77 +174,51 @@ conv3d_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
   const int sp_tiles = g.tiles_h * g.tiles_w;
   const long long total_tiles = static_cast<long long>(g.b) * g.t * sp_tiles * g.n_tiles;
 
-  if (warp == 0 && elect_one()) {   // elect.sync: the compiler keeps the role's code on the uniform datapath
-    // ===== TMA producer =====
-    int stage = 0;
-    uint32_t phase = 0;
-    const int ph = g.kh >> 1, pw = g.kw >> 1;
-    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int nt = static_cast<int>(tile % g.n_tiles);
-      long long r = tile / g.n_tiles;
-      const int sp = static_cast<int>(r % sp_tiles);
-      r /= sp_tiles;
-      const int tt = static_cast<int>(r % g.t);
-      const int bb = static_cast<int>(r / g.t);
-      const int h0 = (sp / g.tiles_w) * g.th, w0 = (sp % g.tiles_w) * g.tw;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        // K order (dt, dh, channel chunk, dw): the same accumulation order as the kw-reuse kernel, so which kernel a call
-        // is dispatched to (it depends on the number of tiles, i.e. on the temporal chunking) never changes the bits
-        const int grp = kb / g.kw;
-        const int dw = kb - grp * g.kw;
-        const int dtdh = grp / cchunks;
-        const int cc = grp - dtdh * cchunks;
-        const int dt = dtdh / g.kh, dh = dtdh - dt * g.kh;
-        const int wk = (dtdh * g.kw + dw) * cchunks + cc;     // K block of tap (dt, dh, dw), chunk cc in the weight matrix
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-        mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-        tma_load_5d(sa, &tm_x, &full_bar[stage], cc * CBK, w0 * g.sw + dw - pw, h0 * g.sh + dh - ph, tt * g.st + dt, bb);
-        tma_load_2d(sa + Cfg::A_BYTES, &tm_w, &full_bar[stage], wk * CBK, nt * BN);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
+  if (wgroup == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
+      // ===== TMA producer =====
+      int stage = 0;
+      uint32_t phase = 0;
+      const int ph = g.kh >> 1, pw = g.kw >> 1;
+      for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const int nt = static_cast<int>(tile % g.n_tiles);
+        long long r = tile / g.n_tiles;
+        const int sp = static_cast<int>(r % sp_tiles);
+        r /= sp_tiles;
+        const int tt = static_cast<int>(r % g.t);
+        const int bb = static_cast<int>(r / g.t);
+        const int h0 = (sp / g.tiles_w) * g.th, w0 = (sp % g.tiles_w) * g.tw;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          // K order (dt, dh, channel chunk, dw)
+          const int grp = kb / g.kw;
+          const int dw = kb - grp * g.kw;
+          const int dtdh = grp / cchunks;
+          const int cc = grp - dtdh * cchunks;
+          const int dt = dtdh / g.kh, dh = dtdh - dt * g.kh;
+          const int wk = (dtdh * g.kw + dw) * cchunks + cc;     // K block of tap (dt, dh, dw), chunk cc in the weight matrix
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
+          mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+          tma_load_5d(sa, &tm_x, &full_bar[stage], cc * CBK, w0 * g.sw + dw - pw, h0 * g.sh + dh - ph, tt * g.st + dt, bb);
+          tma_load_2d(sa + Cfg::A_BYTES, &tm_w, &full_bar[stage], wk * CBK, nt * BN);
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
         }
       }
     }
-  } else if (warp == 1 && elect_one()) {
-    // ===== MMA issuer =====
-    constexpr uint32_t idesc = make_idesc_bf16(CBM, BN, 0, 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + acc * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-        const uint64_t da = make_smem_desc_kmajor_sw128(sa);
-        const uint64_t db = make_smem_desc_kmajor_sw128(sa + Cfg::A_BYTES);
-#pragma unroll
-        for (int kk = 0; kk < CBK / 16; ++kk) umma_ss(tmem_d, da + 2 * kk, db + 2 * kk, idesc, (kb | kk) != 0 ? 1u : 0u);
-        umma_commit(&empty_bar[stage]);
-        if (kb == num_kb - 1) umma_commit(&tmem_full_bar[acc]);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue: thread == output voxel =====
-    const int q = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const int rrow = q * 32 + lane;
+  } else {
+    // ===== consumers: K loop on the tensor cores, then the epilogue (thread == output voxel x channel-chunk parity) =====
+    setmaxnreg_inc<232>();
+    const int wg = wgroup - 1;
+    const int tid = threadIdx.x & 127;
+    const int rrow = wg * 64 + (tid & 63);
     const int lh = rrow / g.tw, lw = rrow - lh * g.tw;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[BN / 2];
     for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int nt = static_cast<int>(tile % g.n_tiles);
       long long r = tile / g.n_tiles;
@@ -278,439 +228,31 @@ conv3d_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
       const int bb = static_cast<int>(r / g.t);
       const int hh = (sp / g.tiles_w) * g.th + lh, ww = (sp % g.tiles_w) * g.tw + lw;
       const bool valid = hh < g.h && ww < g.w;
-      const int n_base = nt * BN;
-
-      mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BN;
-      conv_epilogue_tile<BN>(g, taddr, bb, tt, hh, ww, valid, n_base);
-      tc_fence_before();
-      mbar_arrive(&tmem_empty_bar[acc]);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
+      pipe_consume_tile<BN>(acc, smem, full_bar, empty_bar, num_kb, wg, stage, phase);
+      named_bar_sync(1 + wg, 128);   // the previous tile's epilogue reads of this warpgroup's staging rows are done
+      pipe_stage_acc<BN>(acc, acc_tile, wg);
+      named_bar_sync(1 + wg, 128);
+      conv_epilogue_tile<BN>(g, acc_tile + rrow * Cfg::ACC_PITCH, tid >> 6, bb, tt, hh, ww, valid, nt * BN);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// 2-CTA variant: a CTA pair computes two spatially adjacent 128-voxel patches x BN channels with ONE 256-row MMA; each CTA
-// loads its own input box and half of the weight tile (protocol as gemm2_bf16_tc_kernel in pf_gemm.cu).
-// ---------------------------------------------------------------------------------------------------------------
-template <int BN>
-struct Conv2Cfg {
-  static constexpr int A_BYTES = CBM * CBK * 2;
-  static constexpr int B_BYTES = (BN / 2) * CBK * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BN >= 256) ? 6 : 8;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;
-  static constexpr int TMEM_COLS = (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-};
-
-template <int BN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(CONV_THREADS, 1)
-conv3d2_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w, const ConvArgs g) {
-  using Cfg = Conv2Cfg<BN>;
-  constexpr int STAGES = Cfg::STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-
-  __shared__ __align__(8) uint64_t full_bar[STAGES];
-  __shared__ __align__(8) uint64_t empty_bar[STAGES];
-  __shared__ __align__(8) uint64_t tmem_full_bar[2];
-  __shared__ __align__(8) uint64_t tmem_empty_bar[2];
-  __shared__ uint32_t tmem_base_slot;
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tm_x);
-    tma_prefetch_desc(&tm_w);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full_bar[i], 2);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full_bar[i], 1);
-      mbar_init(&tmem_empty_bar[i], 256);
-    }
-    fence_barrier_init();
-  }
-  cluster_sync_all();
-  if (warp == 2) {
-    tmem_alloc2(&tmem_base_slot, Cfg::TMEM_COLS);
-    tmem_relinquish2();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_slot;
-
-  const int cchunks = g.cin / CBK;
-  const int num_kb = g.taps * cchunks;
-  const int sp_tiles = g.tiles_h * g.tiles_w;
-  const int sp_pairs = (sp_tiles + 1) / 2;
-  const long long total_tiles = static_cast<long long>(g.b) * g.t * sp_pairs * g.n_tiles;
-  const int cluster_id = blockIdx.x >> 1;
-  const int num_clusters = gridDim.x >> 1;
-
-  // decode: n tile fastest, then patch pair, frame, batch; this CTA owns patch 2*pair + rank (may fall off the end)
-  auto decode = [&](long long tile, int& nt, int& tt, int& bb, int& h0, int& w0) {
-    nt = static_cast<int>(tile % g.n_tiles);
-    long long r = tile / g.n_tiles;
-    const int sp = static_cast<int>(r % sp_pairs) * 2 + static_cast<int>(rank);
-    r /= sp_pairs;
-    tt = static_cast<int>(r % g.t);
-    bb = static_cast<int>(r / g.t);
-    if (sp < sp_tiles) {
-      h0 = (sp / g.tiles_w) * g.th;
-      w0 = (sp % g.tiles_w) * g.tw;
-    } else {
-      h0 = g.h + g.th;   // entirely outside: TMA zero-fills, the epilogue stores nothing
-      w0 = 0;
-    }
-  };
-
-  if (warp == 0 && elect_one()) {
-    int stage = 0;
-    uint32_t phase = 0;
-    const int ph = g.kh >> 1, pw = g.kw >> 1;
-    for (long long tile = cluster_id; tile < total_tiles; tile += num_clusters) {
-      int nt, tt, bb, h0, w0;
-      decode(tile, nt, tt, bb, h0, w0);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        // K order (dt, dh, channel chunk, dw): the same accumulation order as the kw-reuse kernel, so which kernel a call
-        // is dispatched to (it depends on the number of tiles, i.e. on the temporal chunking) never changes the bits
-        const int grp = kb / g.kw;
-        const int dw = kb - grp * g.kw;
-        const int dtdh = grp / cchunks;
-        const int cc = grp - dtdh * cchunks;
-        const int dt = dtdh / g.kh, dh = dtdh - dt * g.kh;
-        const int wk = (dtdh * g.kw + dw) * cchunks + cc;     // K block of tap (dt, dh, dw), chunk cc in the weight matrix
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-        if (leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * Cfg::STAGE_BYTES);
-        else mbar_arrive_remote(&full_bar[stage], 0);
-        tma_load_5d_2cta(sa, &tm_x, &full_bar[stage], cc * CBK, w0 * g.sw + dw - pw, h0 * g.sh + dh - ph, tt * g.st + dt, bb);
-        tma_load_2d_2cta(sa + Cfg::A_BYTES, &tm_w, &full_bar[stage], wk * CBK, nt * BN + static_cast<int>(rank) * (BN / 2));
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-  } else if (warp == 1 && leader && elect_one()) {
-    constexpr uint32_t idesc = make_idesc_bf16(2 * CBM, BN, 0, 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (long long tile = cluster_id; tile < total_tiles; tile += num_clusters) {
-      mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + acc * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-        const uint64_t da = make_smem_desc_kmajor_sw128(sa);
-        const uint64_t db = make_smem_desc_kmajor_sw128(sa + Cfg::A_BYTES);
-#pragma unroll
-        for (int kk = 0; kk < CBK / 16; ++kk) umma_ss_2cta(tmem_d, da + 2 * kk, db + 2 * kk, idesc, (kb | kk) != 0 ? 1u : 0u);
-        umma_commit_2cta(&empty_bar[stage]);
-        if (kb == num_kb - 1) umma_commit_2cta(&tmem_full_bar[acc]);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
-  } else if (warp >= 4) {
-    const int q = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const int rrow = q * 32 + lane;
-    const int lh = rrow / g.tw, lw = rrow - lh * g.tw;
-    for (long long tile = cluster_id; tile < total_tiles; tile += num_clusters) {
-      int nt, tt, bb, h0, w0;
-      decode(tile, nt, tt, bb, h0, w0);
-      const int hh = h0 + lh, ww = w0 + lw;
-      const bool valid = hh < g.h && ww < g.w;
-      mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BN;
-      conv_epilogue_tile<BN>(g, taddr, bb, tt, hh, ww, valid, nt * BN);
-      tc_fence_before();
-      if (leader) mbar_arrive(&tmem_empty_bar[acc]);
-      else mbar_arrive_remote(&tmem_empty_bar[acc], 0);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, Cfg::TMEM_COLS);
-  }
-}
-
-template <int BN>
-static int launch_conv2(const CUtensorMap& tm_x, const CUtensorMap& tm_w, const ConvArgs& g, cudaStream_t stream) {
-  using Cfg = Conv2Cfg<BN>;
-  auto kern = conv3d2_tc_kernel<BN>;
-  if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), Cfg::SMEM_BYTES, "conv2")) return rc;
-  const int sp_pairs = (g.tiles_h * g.tiles_w + 1) / 2;
-  const long long total = static_cast<long long>(g.b) * g.t * sp_pairs * g.n_tiles;
-  int sms = num_sms();
-  if (sms <= 0) sms = 148;
-  long long clusters = sms / 2;
-  if (total < clusters) clusters = total;
-  kern<<<static_cast<int>(2 * clusters), CONV_THREADS, Cfg::SMEM_BYTES, stream>>>(tm_x, tm_w, g);
-  return check_launch("pf_causal_conv3d(2cta)");
-}
-
-template <int BN>
-struct Conv2wCfg {
-  // kw-tap reuse: ONE haloed input row of 128 + 2 voxels (x 64 channels) per (kt, kh, channel chunk) feeds the three kw
-  // taps -- the A descriptor of tap kw starts kw rows (kw * 128 B) into the tile -- so the input patch crosses L2 -> smem
-  // 9x instead of 27x (ncu on the 128->128 full-resolution conv: tensor pipe 46 %, operand traffic bound).
-  static constexpr int A_ROWS = CBM + 2;
-  static constexpr int A_TX = A_ROWS * CBK * 2;                   // bytes the TMA delivers
-  static constexpr int A_BYTES = (A_TX + 1023) / 1024 * 1024;     // padded: the weight tiles stay 1024-aligned
-  static constexpr int B_BYTES = (BN / 2) * CBK * 2;              // one tap, this CTA's half of the filters
-  static constexpr int STAGE_BYTES = A_BYTES + 3 * B_BYTES;
-  static constexpr int STAGES = (226 * 1024) / STAGE_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;
-  static constexpr int TMEM_COLS = (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-};
-
-template <int BN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(CONV_THREADS, 1)
-conv3d2w_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w, const ConvArgs g) {
-  using Cfg = Conv2wCfg<BN>;
-  constexpr int STAGES = Cfg::STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-
-  __shared__ __align__(8) uint64_t full_bar[STAGES];
-  __shared__ __align__(8) uint64_t empty_bar[STAGES];
-  __shared__ __align__(8) uint64_t tmem_full_bar[2];
-  __shared__ __align__(8) uint64_t tmem_empty_bar[2];
-  __shared__ uint32_t tmem_base_slot;
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tm_x);
-    tma_prefetch_desc(&tm_w);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full_bar[i], 2);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full_bar[i], 1);
-      mbar_init(&tmem_empty_bar[i], 256);
-    }
-    fence_barrier_init();
-  }
-  cluster_sync_all();
-  if (warp == 2) {
-    tmem_alloc2(&tmem_base_slot, Cfg::TMEM_COLS);
-    tmem_relinquish2();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_slot;
-
-  const int cchunks = g.cin / CBK;
-  const int num_grp = g.kt * g.kh * cchunks;   // (dt, dh, channel chunk) groups, three kw taps each
-  const int sp_tiles = g.tiles_h * g.tiles_w;
-  const int sp_pairs = (sp_tiles + 1) / 2;
-  const long long total_tiles = static_cast<long long>(g.b) * g.t * sp_pairs * g.n_tiles;
-  const int cluster_id = blockIdx.x >> 1;
-  const int num_clusters = gridDim.x >> 1;
-
-  // decode: n tile fastest, then patch pair, frame, batch; this CTA owns patch 2*pair + rank (may fall off the end)
-  auto decode = [&](long long tile, int& nt, int& tt, int& bb, int& h0, int& w0) {
-    nt = static_cast<int>(tile % g.n_tiles);
-    long long r = tile / g.n_tiles;
-    const int sp = static_cast<int>(r % sp_pairs) * 2 + static_cast<int>(rank);
-    r /= sp_pairs;
-    tt = static_cast<int>(r % g.t);
-    bb = static_cast<int>(r / g.t);
-    if (sp < sp_tiles) {
-      h0 = (sp / g.tiles_w) * g.th;
-      w0 = (sp % g.tiles_w) * g.tw;
-    } else {
-      h0 = g.h + g.th;   // entirely outside: TMA zero-fills, the epilogue stores nothing
-      w0 = 0;
-    }
-  };
-
-  if (warp == 0 && elect_one()) {
-    int stage = 0;
-    uint32_t phase = 0;
-    const int ph = g.kh >> 1, pw = g.kw >> 1;
-    for (long long tile = cluster_id; tile < total_tiles; tile += num_clusters) {
-      int nt, tt, bb, h0, w0;
-      decode(tile, nt, tt, bb, h0, w0);
-      for (int grp = 0; grp < num_grp; ++grp) {
-        const int dtdh = grp / cchunks;
-        const int cc = grp - dtdh * cchunks;
-        const int dt = dtdh / g.kh, dh = dtdh - dt * g.kh;
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-        if (leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * (Cfg::A_TX + 3 * Cfg::B_BYTES));
-        else mbar_arrive_remote(&full_bar[stage], 0);
-        tma_load_5d_2cta(sa, &tm_x, &full_bar[stage], cc * CBK, w0 - pw, h0 + dh - ph, tt + dt, bb);   // 130 voxels
-#pragma unroll
-        for (int kw = 0; kw < 3; ++kw) {
-          const int kb = (dtdh * 3 + kw) * cchunks + cc;        // K block of tap (dt, dh, kw), channel chunk cc
-          tma_load_2d_2cta(sa + Cfg::A_BYTES + kw * Cfg::B_BYTES, &tm_w, &full_bar[stage], kb * CBK,
-                           nt * BN + static_cast<int>(rank) * (BN / 2));
-        }
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-  } else if (warp == 1 && leader && elect_one()) {
-    constexpr uint32_t idesc = make_idesc_bf16(2 * CBM, BN, 0, 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (long long tile = cluster_id; tile < total_tiles; tile += num_clusters) {
-      mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + acc * BN;
-      for (int grp = 0; grp < num_grp; ++grp) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-#pragma unroll
-        for (int kw = 0; kw < 3; ++kw) {
-          // rows [kw, kw + 128) of the haloed tile: start address advanced by kw 128-byte rows inside the 1024-byte swizzle
-          // atom.  The swizzle is applied on absolute smem address bits, so the advanced descriptor reads exactly what
-          // the TMA wrote; the base-offset field [49,52) must stay 0 (pinned on hardware: tools/gpu_check.py probe_rowoff)
-          const uint64_t da = make_smem_desc_kmajor_sw128(sa + kw * 128) | (static_cast<uint64_t>(g.kw_baseoff ? kw : 0) << 49);
-          const uint64_t db = make_smem_desc_kmajor_sw128(sa + Cfg::A_BYTES + kw * Cfg::B_BYTES);
-#pragma unroll
-          for (int kk = 0; kk < CBK / 16; ++kk)
-            umma_ss_2cta(tmem_d, da + 2 * kk, db + 2 * kk, idesc, (grp | kw | kk) != 0 ? 1u : 0u);
-        }
-        umma_commit_2cta(&empty_bar[stage]);
-        if (grp == num_grp - 1) umma_commit_2cta(&tmem_full_bar[acc]);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
-  } else if (warp >= 4) {
-    const int q = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const int rrow = q * 32 + lane;
-    const int lh = rrow / g.tw, lw = rrow - lh * g.tw;
-    for (long long tile = cluster_id; tile < total_tiles; tile += num_clusters) {
-      int nt, tt, bb, h0, w0;
-      decode(tile, nt, tt, bb, h0, w0);
-      const int hh = h0 + lh, ww = w0 + lw;
-      const bool valid = hh < g.h && ww < g.w;
-      mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BN;
-      conv_epilogue_tile<BN>(g, taddr, bb, tt, hh, ww, valid, nt * BN);
-      tc_fence_before();
-      if (leader) mbar_arrive(&tmem_empty_bar[acc]);
-      else mbar_arrive_remote(&tmem_empty_bar[acc], 0);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, Cfg::TMEM_COLS);
-  }
-}
-
-template <int BN>
-static int launch_conv2w(const CUtensorMap& tm_x, const CUtensorMap& tm_w, const ConvArgs& g, cudaStream_t stream) {
-  using Cfg = Conv2wCfg<BN>;
-  auto kern = conv3d2w_tc_kernel<BN>;
-  if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), Cfg::SMEM_BYTES, "conv2")) return rc;
-  const int sp_pairs = (g.tiles_h * g.tiles_w + 1) / 2;
-  const long long total = static_cast<long long>(g.b) * g.t * sp_pairs * g.n_tiles;
-  int sms = num_sms();
-  if (sms <= 0) sms = 148;
-  long long clusters = sms / 2;
-  if (total < clusters) clusters = total;
-  kern<<<static_cast<int>(2 * clusters), CONV_THREADS, Cfg::SMEM_BYTES, stream>>>(tm_x, tm_w, g);
-  return check_launch("pf_causal_conv3d(2cta, kw reuse)");
 }
 
 template <int BN>
 static int launch_conv(const CUtensorMap& tm_x, const CUtensorMap& tm_w, const ConvArgs& g, cudaStream_t stream) {
-  using Cfg = ConvCfg<BN>;
-  auto kern = conv3d_tc_kernel<BN>;
+  using Cfg = PipeCfg<BN>;
+  auto kern = conv3d_wgmma_kernel<BN>;
   if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), Cfg::SMEM_BYTES, "conv")) return rc;
   const long long total = static_cast<long long>(g.b) * g.t * g.tiles_h * g.tiles_w * g.n_tiles;
   int grid = num_sms();
-  if (grid <= 0) grid = 148;
+  if (grid <= 0) grid = 132;
   if (total < grid) grid = static_cast<int>(total);
-  kern<<<grid, CONV_THREADS, Cfg::SMEM_BYTES, stream>>>(tm_x, tm_w, g);
+  kern<<<grid, PIPE_THREADS, Cfg::SMEM_BYTES, stream>>>(tm_x, tm_w, g);
   return check_launch("pf_causal_conv3d");
 }
 
 int warmup_conv() {
-  int rc = 0;
-#define PF_WARM(KERN, CFG) if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(KERN), CFG::SMEM_BYTES, #KERN)
-  PF_WARM((conv3d_tc_kernel<256>), ConvCfg<256>);
-  PF_WARM((conv3d_tc_kernel<128>), ConvCfg<128>);
-  PF_WARM((conv3d_tc_kernel<64>), ConvCfg<64>);
-  PF_WARM((conv3d2_tc_kernel<256>), Conv2Cfg<256>);
-  PF_WARM((conv3d2_tc_kernel<128>), Conv2Cfg<128>);
-  PF_WARM((conv3d2w_tc_kernel<256>), Conv2wCfg<256>);
-  PF_WARM((conv3d2w_tc_kernel<128>), Conv2wCfg<128>);
-#undef PF_WARM
+  int rc = ensure_dyn_smem(reinterpret_cast<const void*>(conv3d_wgmma_kernel<128>), PipeCfg<128>::SMEM_BYTES, "conv<128>");
+  if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(conv3d_wgmma_kernel<64>), PipeCfg<64>::SMEM_BYTES, "conv<64>");
   return rc;
 }
 
@@ -743,8 +285,7 @@ extern "C" int pf_causal_conv3d(const pf_conv3d_desc* d, void* stream_) {
   g.tw = tw; g.th = 128 / tw;
   g.tiles_w = (d->w + g.tw - 1) / g.tw;
   g.tiles_h = (d->h + g.th - 1) / g.th;
-  const int bn = (d->cout % 256 == 0) ? 256 : (d->cout % 128 == 0) ? 128 : 64;
-  g.n_tiles = d->cout / bn;
+  int bn = (d->cout % 128 == 0) ? 128 : 64;
   g.bias = d->bias;
   g.store_mode = d->store_mode;
   g.out = d->out; g.out_f32 = d->out_f32;
@@ -756,22 +297,13 @@ extern "C" int pf_causal_conv3d(const pf_conv3d_desc* d, void* stream_) {
   g.residual = static_cast<const __nv_bfloat16*>(d->residual);
   g.res_t_total = d->res_t_total; g.res_t_offset = d->res_t_offset;
 
-  // 2-CTA tiles when there is enough work for 74 CTA pairs; kernel_variant pins a kernel (tests)
-  PF_REQUIRE(d->kernel_variant >= 0 && d->kernel_variant <= 3, "pf_causal_conv3d: bad kernel_variant %d", d->kernel_variant);
-  bool two_cta = bn >= 128 && static_cast<long long>(d->b) * d->t * g.tiles_h * g.tiles_w * g.n_tiles >= 296;
-  if (d->kernel_variant == 1) two_cta = false;
-  if (d->kernel_variant >= 2) {
-    PF_REQUIRE(bn >= 128, "pf_causal_conv3d: kernel_variant %d (2-CTA) needs cout %% 128 == 0", d->kernel_variant);
-    two_cta = true;
-  }
+  // kernel_variant 1 / 2 pins the 128-wide / 64-wide filter tile (same K order, same bits)
+  PF_REQUIRE(d->kernel_variant >= 0 && d->kernel_variant <= 2, "pf_causal_conv3d: bad kernel_variant %d", d->kernel_variant);
+  PF_REQUIRE(d->kernel_variant != 1 || bn == 128, "pf_causal_conv3d: kernel_variant 1 (128-wide filter tiles) needs cout %% 128 == 0");
+  if (d->kernel_variant == 2) bn = 64;
+  g.n_tiles = d->cout / bn;
   // input geometry: (t-1)*st + kt frames (the kt-1 causal frames physically first), h*sh x w*sw voxels (symmetric pad 1 is
   // the TMA's out-of-bounds zero fill).  A strided conv loads every sh-th / sw-th voxel of a (th*sh) x (tw*sw) box.
-  // kw-tap reuse (conv3d2w): full 128-voxel rows, 3x3x3, unit stride.
-  // Measured on B200: 128->128 on 2x768x1280 1.65 -> 1.01 ms (1057 -> 1724 TFLOP/s), 256->256 on 2x384x640 1765 -> 1888.
-  const bool kwr_ok = g.th == 1 && g.tw == 128 && d->kt == 3 && d->kh == 3 && st == 1 && sh == 1;
-  if (d->kernel_variant == 3) PF_REQUIRE(kwr_ok, "pf_causal_conv3d: kernel_variant 3 (kw reuse) needs w > 64, a 3x3x3 kernel and unit stride");
-  const bool kwr = two_cta && kwr_ok && d->kernel_variant != 2;
-  g.kw_baseoff = 0;   // the UMMA descriptor's base-offset field must stay 0 (pinned by the probe, tools/gpu_check.py probe_rowoff)
   const int tin = (d->t - 1) * st + d->kt;
   const int hin = d->h * sh, win = d->w * sw;
   CUtensorMap tm_x, tm_w;
@@ -780,7 +312,7 @@ extern "C" int pf_causal_conv3d(const pf_conv3d_desc* d, void* stream_) {
                               static_cast<uint64_t>(tin), static_cast<uint64_t>(d->b)};
     const uint64_t s0 = static_cast<uint64_t>(d->cin) * 2;
     const uint64_t strides[4] = {s0, s0 * win, s0 * win * hin, s0 * win * hin * tin};
-    const uint32_t box[5] = {CBK, static_cast<uint32_t>(kwr ? g.tw + 2 : g.tw * sw), static_cast<uint32_t>(g.th * sh), 1, 1};
+    const uint32_t box[5] = {CBK, static_cast<uint32_t>(g.tw * sw), static_cast<uint32_t>(g.th * sh), 1, 1};
     const uint32_t estr[5] = {1, static_cast<uint32_t>(sw), static_cast<uint32_t>(sh), 1, 1};
     int rc = encode_tensor_map(&tm_x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, d->x, dims, strides, box,
                                CU_TENSOR_MAP_SWIZZLE_128B, estr);
@@ -790,22 +322,11 @@ extern "C" int pf_causal_conv3d(const pf_conv3d_desc* d, void* stream_) {
     const uint64_t kdim = static_cast<uint64_t>(g.taps) * d->cin;
     const uint64_t dims[2] = {kdim, static_cast<uint64_t>(d->cout)};
     const uint64_t strides[1] = {kdim * 2};
-    const uint32_t box[2] = {CBK, static_cast<uint32_t>(two_cta ? bn / 2 : bn)};
+    const uint32_t box[2] = {CBK, static_cast<uint32_t>(bn)};
     int rc = encode_tensor_map(&tm_w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, d->wgt, dims, strides, box,
                                CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
-  if (kwr) {
-    if (bn == 256) return launch_conv2w<256>(tm_x, tm_w, g, stream);
-    return launch_conv2w<128>(tm_x, tm_w, g, stream);
-  }
-  if (two_cta) {
-    if (bn == 256) return launch_conv2<256>(tm_x, tm_w, g, stream);
-    return launch_conv2<128>(tm_x, tm_w, g, stream);
-  }
-  switch (bn) {
-    case 256: return launch_conv<256>(tm_x, tm_w, g, stream);
-    case 128: return launch_conv<128>(tm_x, tm_w, g, stream);
-    default: return launch_conv<64>(tm_x, tm_w, g, stream);
-  }
+  if (bn == 128) return launch_conv<128>(tm_x, tm_w, g, stream);
+  return launch_conv<64>(tm_x, tm_w, g, stream);
 }

@@ -1,13 +1,13 @@
-// pf_gemm.cu — persistent warp-specialised bf16 GEMM on tcgen05 tensor cores with fused epilogues.
+// pf_gemm.cu — persistent warp-specialised bf16 GEMM on Hopper warpgroup MMA (wgmma) with fused epilogues.
 //
 //   out = epilogue(A[rows, K] . W[N, K]^T + bias)
 //
-// One CTA per SM (persistent, static tile schedule), 256 threads:
-//   warp 0 (one lane)  TMA producer: A tile [128 x 64] + W tile [BN x 64] per stage, SWIZZLE_128B, mbarrier tx-count
-//   warp 1 (one lane)  MMA issuer  : 4 x tcgen05.mma (128 x BN x 16) per stage, fp32 accumulators in TMEM,
-//                                    tcgen05.commit releases the smem stage / publishes the accumulator
-//   warp 2             TMEM allocator (2 accumulator buffers -> epilogue of tile i overlaps MMA of tile i+1)
-//   warps 4..7         epilogue: tcgen05.ld (lane == output row), fused elementwise math, vectorised global stores
+// One CTA per SM (persistent, static tile schedule), 384 threads (pf_common.cuh "shared TMA -> wgmma pipeline"):
+//   warpgroup 0 (one lane)  TMA producer: A tile [128 x 64] + W tile [BN x 64] per stage, SWIZZLE_128B, mbarrier tx-count
+//   warpgroups 1, 2         consumers: 4 x wgmma.mma_async (64 x BN x 16) per stage each, fp32 accumulators in registers;
+//                           after the K loop the fragments are staged through shared memory so that the epilogue runs with one
+//                           thread per output row (64 rows x 2 column halves per warpgroup) and stores whole row segments
+// The producer runs ahead into the next tile's stages while the consumers are in the epilogue.
 //
 // Epilogues (include/pf_b200.h PF_EPI_*): bias / GELU-tanh / fp32 store / gate*x+residual / per-head RMSNorm + RoPE
 // with head-major Q,K,V stores / the single-block fused q|k|v|mlp split.
@@ -23,7 +23,6 @@ struct GemmArgs {
   int batches, row_begin, row_count;
   int n, k;
   int m_tiles, n_tiles;
-  int n_begin;   // first output column of this launch (a GEMM may be issued as a 256-wide main part + a narrower tail)
   const float* bias;
   void* out;
   long long ldo;
@@ -42,22 +41,11 @@ struct GemmArgs {
   // sequence parallel: q/k/v heads go straight into the owning rank's [3][peer_heads][peer_seq][64] buffer (pf_b200.h)
   __nv_bfloat16* peer_qkv[PF_MAX_PEERS];
   int peer_count, peer_heads, peer_seq, peer_row0;
-  int epi_staged;   // GATE_RESID: transposed read-modify-write through shared memory (pf_set_option(PF_OPT_GEMM_STAGED_RESID))
+  int epi_staged;   // GATE_RESID: whole-row read-modify-write, one warp per row segment (pf_set_option(PF_OPT_GEMM_STAGED_RESID))
 };
 
-constexpr int BM = 128;
-constexpr int BK = 64;
-constexpr int GEMM_THREADS = 256;
-
-template <int BN>
-struct GemmCfg {
-  static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = BN * BK * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BN >= 256) ? 4 : (BN >= 192) ? 5 : (BN >= 128) ? 6 : 8;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;
-  static constexpr int TMEM_COLS = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-};
+constexpr int BM = PIPE_BM;
+constexpr int BK = PIPE_BK;
 
 // ---- epilogue helpers (one thread == one output row) -----------------------
 __device__ __forceinline__ void store_bf16x32(__nv_bfloat16* dst, const float (&x)[32]) {
@@ -73,38 +61,29 @@ __device__ __forceinline__ void store_bf16x32(__nv_bfloat16* dst, const float (&
   }
 }
 
-__device__ __forceinline__ void add_bias32(float (&x)[32], const uint32_t (&v)[32], const float* bias) {
-  if (bias != nullptr) {
-    const float4* b4 = reinterpret_cast<const float4*>(bias);
+// x[0..32) = staged accumulators + bias
+__device__ __forceinline__ void load_bias32(float (&x)[32], const float* srow, const float* bias) {
+  const float4* s4 = reinterpret_cast<const float4*>(srow);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float4 b = __ldg(b4 + i);
-      x[4 * i + 0] = __uint_as_float(v[4 * i + 0]) + b.x;
-      x[4 * i + 1] = __uint_as_float(v[4 * i + 1]) + b.y;
-      x[4 * i + 2] = __uint_as_float(v[4 * i + 2]) + b.z;
-      x[4 * i + 3] = __uint_as_float(v[4 * i + 3]) + b.w;
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) x[i] = __uint_as_float(v[i]);
+  for (int i = 0; i < 8; ++i) {
+    const float4 v = s4[i];
+    float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (bias != nullptr) b = __ldg(reinterpret_cast<const float4*>(bias) + i);
+    x[4 * i + 0] = v.x + b.x;
+    x[4 * i + 1] = v.y + b.y;
+    x[4 * i + 2] = v.z + b.z;
+    x[4 * i + 3] = v.w + b.w;
   }
 }
 
-// One head (64 columns = two 32-column TMEM chunks) of q / k / v for one token.
+// One head (64 columns) of q / k / v for one token; `srow` = this token's staged accumulators at the head's first column.
 // section 0 = q, 1 = k (RMSNorm over the head N:66-79, then RoPE B:34-39), 2 = v (plain store).
-// `cs` = this token's RoPE row (16 float4 = (cos, sin) of the 32 rotation pairs), loaded ONCE per output tile by the
-// caller: it depends on the position only, and fetching it inside every head call left its L2 latency exposed 4x per tile.
-__device__ __forceinline__ void qkv_head_epilogue(const GemmArgs& g, uint32_t taddr, int n0, int b, int pos,
-                                                  bool valid, const float4 (&cs_row)[16], bool have_rope) {
-  uint32_t v0[32], v1[32];
-  tmem_ld32(taddr, v0);
-  tmem_ld32(taddr + 32, v1);
-  tmem_ld_wait();
+__device__ __forceinline__ void qkv_head_epilogue(const GemmArgs& g, const float* srow, int n0, int b, int pos, bool valid) {
   float x[64];
   {
     float lo[32], hi[32];
-    add_bias32(lo, v0, g.bias ? g.bias + n0 : nullptr);
-    add_bias32(hi, v1, g.bias ? g.bias + n0 + 32 : nullptr);
+    load_bias32(lo, srow, g.bias ? g.bias + n0 : nullptr);
+    load_bias32(hi, srow + 32, g.bias ? g.bias + n0 + 32 : nullptr);
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
       x[i] = lo[i];
@@ -135,10 +114,11 @@ __device__ __forceinline__ void qkv_head_epilogue(const GemmArgs& g, uint32_t ta
       x[4 * i + 2] *= r * w.z;
       x[4 * i + 3] *= r * w.w;
     }
-    if (have_rope) {
+    if (g.rope != nullptr && valid) {
+      const float4* cs4 = reinterpret_cast<const float4*>(g.rope + static_cast<size_t>(pos) * 64);
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
-        const float4 cs = cs_row[i];  // (cos_{2i}, sin_{2i}, cos_{2i+1}, sin_{2i+1})
+        const float4 cs = __ldg(cs4 + i);  // (cos_{2i}, sin_{2i}, cos_{2i+1}, sin_{2i+1})
         const float a0 = x[4 * i + 0], a1 = x[4 * i + 1], a2 = x[4 * i + 2], a3 = x[4 * i + 3];
         x[4 * i + 0] = cs.x * a0 - cs.y * a1;
         x[4 * i + 1] = cs.y * a0 + cs.x * a1;
@@ -166,448 +146,178 @@ __device__ __forceinline__ void qkv_head_epilogue(const GemmArgs& g, uint32_t ta
   }
 }
 
-// Epilogue of one 128-row accumulator slice: this thread owns output row `m` (TMEM lane), columns [n_base, n_base + BN).
-// `stage`: this warp's 32 x EPI_PITCH fp32 staging block in shared memory (GATE_RESID only): the accumulators arrive one
-// thread per ROW (TMEM lane); the read-modify-write of the fp32 residual stream is done transposed, 8 lanes per row
-// (4 rows x 128 contiguous bytes per warp instruction instead of 32 rows x 16 bytes).
-constexpr int EPI_PITCH = 36;   // floats per staged row: 16-byte aligned, conflict-free for quarter-warp float4 accesses
-
+// Epilogue of one warpgroup's 64-row slice of the staged accumulator tile.  `tid` = thread index in the warpgroup: the
+// row-per-thread forms give thread (row = tid % 64, half = tid / 64) every second 32-column chunk (or 64-column head) of its
+// row; the whole-row GATE_RESID form gives each warp 16 rows and lets its lanes sweep a row's columns, so that the
+// read-modify-write of the fp32 residual stream moves BN * 4 contiguous bytes per warp instruction.
 template <int BN, int EPI>
-__device__ __forceinline__ void epilogue_tile(const GemmArgs& g, uint32_t taddr, int b, int m, int n_base, float* stage) {
+__device__ __forceinline__ void epilogue_tile(const GemmArgs& g, const float* acc_rows, int tid, int b, int m_base, int n_base) {
+  constexpr int PITCH = PipeCfg<BN>::ACC_PITCH;
+  const int row = tid & 63, half = tid >> 6;
+  const int m = m_base + row;
   const bool valid = m < g.row_count;
   const size_t out_row = static_cast<size_t>(b) * g.out_batch_rows + g.out_row_begin + m;
+  const float* srow = acc_rows + row * PITCH;
   bool qkv_tile = (EPI == PF_EPI_QKV_ROPE);
   if (EPI == PF_EPI_QKV_GELU) qkv_tile = n_base < g.n_split;
 
   if (qkv_tile) {
     const int pos = g.out_row_begin + m;
-    const bool have_rope = g.rope != nullptr && valid;
-    float4 cs_row[16];
-    if (have_rope) {
-      const float4* cs4 = reinterpret_cast<const float4*>(g.rope + static_cast<size_t>(pos) * 64);
-#pragma unroll
-      for (int i = 0; i < 16; ++i) cs_row[i] = __ldg(cs4 + i);
-    }
 #pragma unroll 1
-    for (int h = 0; h < BN / 64; ++h) {
-      qkv_head_epilogue(g, taddr + h * 64, n_base + h * 64, b, pos, valid, cs_row, have_rope);
+    for (int h = half; h < BN / 64; h += 2) qkv_head_epilogue(g, srow + h * 64, n_base + h * 64, b, pos, valid);
+  } else if (EPI == PF_EPI_GATE_RESID && g.epi_staged) {
+    constexpr int VEC_PER_ROW = BN / 4, ROWS_PER_IT = 32 / VEC_PER_ROW;
+    const int warp = tid >> 5, lane = tid & 31;
+    const int c4 = lane % VEC_PER_ROW, rsub = lane / VEC_PER_ROW;
+    const float4 gg = __ldg(reinterpret_cast<const float4*>(g.gate + b * g.gate_batch_stride + n_base) + c4);
+    float4 bb = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (g.bias != nullptr) bb = __ldg(reinterpret_cast<const float4*>(g.bias + n_base) + c4);
+    float* obase = reinterpret_cast<float*>(g.out) + g.out_col_begin + n_base + 4 * c4;
+    const size_t row0 = static_cast<size_t>(b) * g.out_batch_rows + g.out_row_begin + m_base;
+#pragma unroll 4
+    for (int it = 0; it < 16 / ROWS_PER_IT; ++it) {
+      const int rr = warp * 16 + it * ROWS_PER_IT + rsub;
+      if (m_base + rr < g.row_count) {
+        const float4 a4 = *reinterpret_cast<const float4*>(acc_rows + rr * PITCH + 4 * c4);
+        float4* dst = reinterpret_cast<float4*>(obase + (row0 + rr) * g.ldo);
+        float4 r4 = *dst;
+        r4.x += gg.x * (a4.x + bb.x);
+        r4.y += gg.y * (a4.y + bb.y);
+        r4.z += gg.z * (a4.z + bb.z);
+        r4.w += gg.w * (a4.w + bb.w);
+        *dst = r4;
+      }
     }
   } else {
 #pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      uint32_t v[32];
-      tmem_ld32(taddr + c * 32, v);
-      tmem_ld_wait();
+    for (int c = half; c < BN / 32; c += 2) {
       const int n0 = n_base + c * 32;
       float x[32];
-      add_bias32(x, v, g.bias ? g.bias + n0 : nullptr);
+      load_bias32(x, srow + c * 32, g.bias ? g.bias + n0 : nullptr);
       if (EPI == PF_EPI_GELU_BF16 || EPI == PF_EPI_QKV_GELU) {
 #pragma unroll
         for (int i = 0; i < 32; ++i) x[i] = gelu_tanh_f(x[i]);
       }
+      if (!valid) continue;
       if (EPI == PF_EPI_STORE_BF16 || EPI == PF_EPI_GELU_BF16 || EPI == PF_EPI_QKV_GELU) {
         const int col = (EPI == PF_EPI_QKV_GELU) ? (g.out_col_begin + n0 - g.n_split) : (g.out_col_begin + n0);
-        if (valid) store_bf16x32(reinterpret_cast<__nv_bfloat16*>(g.out) + out_row * g.ldo + col, x);
+        store_bf16x32(reinterpret_cast<__nv_bfloat16*>(g.out) + out_row * g.ldo + col, x);
       } else if (EPI == PF_EPI_STORE_F32) {
-        if (valid) {
-          float4* d4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(g.out) + out_row * g.ldo +
-                                                 g.out_col_begin + n0);
+        float4* d4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(g.out) + out_row * g.ldo + g.out_col_begin + n0);
 #pragma unroll
-          for (int i = 0; i < 8; ++i) d4[i] = make_float4(x[4 * i], x[4 * i + 1], x[4 * i + 2], x[4 * i + 3]);
-        }
-      } else if (EPI == PF_EPI_GATE_RESID && !g.epi_staged) {
-        // round-1 form: each thread read-modify-writes its own row (32 rows x 16 bytes per warp instruction)
-        if (valid) {
-          float4* d4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(g.out) + out_row * g.ldo +
-                                                 g.out_col_begin + n0);
-          const float4* g4 = reinterpret_cast<const float4*>(g.gate + b * g.gate_batch_stride + n0);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            float4 rr = d4[i];
-            const float4 gg = __ldg(g4 + i);
-            rr.x += gg.x * x[4 * i + 0];
-            rr.y += gg.y * x[4 * i + 1];
-            rr.z += gg.z * x[4 * i + 2];
-            rr.w += gg.w * x[4 * i + 3];
-            d4[i] = rr;
-          }
-        }
+        for (int i = 0; i < 8; ++i) d4[i] = make_float4(x[4 * i], x[4 * i + 1], x[4 * i + 2], x[4 * i + 3]);
       } else if (EPI == PF_EPI_GATE_RESID) {
-        const int lane = threadIdx.x & 31;
-        float4* st4 = reinterpret_cast<float4*>(stage + lane * EPI_PITCH);
+        // each thread read-modify-writes its own row (32 rows x 16 bytes per warp instruction)
+        float4* d4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(g.out) + out_row * g.ldo + g.out_col_begin + n0);
+        const float4* g4 = reinterpret_cast<const float4*>(g.gate + b * g.gate_batch_stride + n0);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) st4[i] = make_float4(x[4 * i], x[4 * i + 1], x[4 * i + 2], x[4 * i + 3]);
-        __syncwarp();
-        const int c4 = lane & 7, rsub = lane >> 3;
-        const float4 gg = __ldg(reinterpret_cast<const float4*>(g.gate + b * g.gate_batch_stride + n0) + c4);
-        const int m0 = m - lane;                               // first row of this warp's 32-row slice
-        float* obase = reinterpret_cast<float*>(g.out) + g.out_col_begin + n0 + 4 * c4;
-        const size_t row0 = static_cast<size_t>(b) * g.out_batch_rows + g.out_row_begin + m0;
-        float4 acc4[8], res4[8];
-#pragma unroll
-        for (int it = 0; it < 8; ++it) {                       // all loads first: 8 independent 128-byte row segments in flight
-          const int rr = it * 4 + rsub;
-          acc4[it] = *reinterpret_cast<const float4*>(stage + rr * EPI_PITCH + 4 * c4);
-          if (m0 + rr < g.row_count) res4[it] = *reinterpret_cast<const float4*>(obase + (row0 + rr) * g.ldo);
+        for (int i = 0; i < 8; ++i) {
+          float4 rr = d4[i];
+          const float4 gg = __ldg(g4 + i);
+          rr.x += gg.x * x[4 * i + 0];
+          rr.y += gg.y * x[4 * i + 1];
+          rr.z += gg.z * x[4 * i + 2];
+          rr.w += gg.w * x[4 * i + 3];
+          d4[i] = rr;
         }
-#pragma unroll
-        for (int it = 0; it < 8; ++it) {
-          const int rr = it * 4 + rsub;
-          if (m0 + rr < g.row_count) {
-            float4 r4 = res4[it];
-            r4.x += gg.x * acc4[it].x;
-            r4.y += gg.y * acc4[it].y;
-            r4.z += gg.z * acc4[it].z;
-            r4.w += gg.w * acc4[it].w;
-            *reinterpret_cast<float4*>(obase + (row0 + rr) * g.ldo) = r4;
-          }
-        }
-        __syncwarp();
       }
     }
   }
 }
 
 template <int BN, int EPI>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
-                    const GemmArgs g) {
-  using Cfg = GemmCfg<BN>;
+__global__ void __launch_bounds__(PIPE_THREADS, 1)
+gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
+                       const GemmArgs g) {
+  using Cfg = PipeCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  float* acc_tile = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
 
   __shared__ __align__(8) uint64_t full_bar[STAGES];
   __shared__ __align__(8) uint64_t empty_bar[STAGES];
-  __shared__ __align__(8) uint64_t tmem_full_bar[2];
-  __shared__ __align__(8) uint64_t tmem_empty_bar[2];
-  __shared__ uint32_t tmem_base_slot;
-  __shared__ __align__(16) float epi_stage[EPI == PF_EPI_GATE_RESID ? 4 * 32 * EPI_PITCH : 4];
 
   const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wgroup = warp >> 2;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_a);
     tma_prefetch_desc(&tm_b);
-  }
-  if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full_bar[i], 1);
-      mbar_init(&tmem_empty_bar[i], 128);
+      mbar_init(&empty_bar[i], PIPE_CONSUMER_WARPS);
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(&tmem_base_slot, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_slot;
 
   const int num_kb = (g.k + BK - 1) / BK;
   const int tiles_per_batch = g.m_tiles * g.n_tiles;
   const int total_tiles = g.batches * tiles_per_batch;
 
-  if (warp == 0 && elect_one()) {   // elect.sync: the compiler keeps the role's code on the uniform datapath
-    // ===== TMA producer =====
+  if (wgroup == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
+      // ===== TMA producer =====
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const int b = tile / tiles_per_batch;
+        const int r = tile - b * tiles_per_batch;
+        const int mt = r / g.n_tiles;
+        const int nt = r - mt * g.n_tiles;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
+          mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+          tma_load_3d(sa, &tm_a, &full_bar[stage], kb * BK, g.row_begin + mt * BM, b);
+          tma_load_2d(sa + Cfg::A_BYTES, &tm_b, &full_bar[stage], kb * BK, nt * BN);
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    }
+  } else {
+    // ===== consumers: K loop on the tensor cores, then the epilogue of their own 64 rows =====
+    setmaxnreg_inc<232>();
+    const int wg = wgroup - 1;
+    const int tid = threadIdx.x & 127;
     int stage = 0;
     uint32_t phase = 0;
+    float acc[BN / 2];
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int b = tile / tiles_per_batch;
       const int r = tile - b * tiles_per_batch;
       const int mt = r / g.n_tiles;
       const int nt = r - mt * g.n_tiles;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-        uint8_t* sb = sa + Cfg::A_BYTES;
-        mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-        tma_load_3d(sa, &tm_a, &full_bar[stage], kb * BK, g.row_begin + mt * BM, b);
-        tma_load_2d(sb, &tm_b, &full_bar[stage], kb * BK, g.n_begin + nt * BN);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-  } else if (warp == 1 && elect_one()) {
-    // ===== MMA issuer =====
-    constexpr uint32_t idesc = make_idesc_bf16(BM, BN, 0, 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + acc * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-        const uint64_t da = make_smem_desc_kmajor_sw128(sa);
-        const uint64_t db = make_smem_desc_kmajor_sw128(sa + Cfg::A_BYTES);
-#pragma unroll
-        for (int kk = 0; kk < BK / 16; ++kk) {
-          // +32 bytes (>>4 = 2) per UMMA_K = 16 bf16 inside the 128-byte swizzle row
-          umma_ss(tmem_d, da + 2 * kk, db + 2 * kk, idesc, (kb | kk) != 0 ? 1u : 0u);
-        }
-        umma_commit(&empty_bar[stage]);
-        if (kb == num_kb - 1) umma_commit(&tmem_full_bar[acc]);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue =====
-    const int q = warp & 3;  // TMEM lane quarter this warp may read
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int b = tile / tiles_per_batch;
-      const int r = tile - b * tiles_per_batch;
-      const int mt = r / g.n_tiles;
-      const int nt = r - mt * g.n_tiles;
-      const int m = mt * BM + q * 32 + lane;
-      const int n_base = g.n_begin + nt * BN;
-
-      mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BN;
-
-      epilogue_tile<BN, EPI>(g, taddr, b, m, n_base, epi_stage + (EPI == PF_EPI_GATE_RESID ? q * 32 * EPI_PITCH : 0));
-      // all tcgen05.ld of this accumulator have completed (wait::ld above) -> hand the buffer back
-      tc_fence_before();
-      mbar_arrive(&tmem_empty_bar[acc]);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
+      pipe_consume_tile<BN>(acc, smem, full_bar, empty_bar, num_kb, wg, stage, phase);
+      named_bar_sync(1 + wg, 128);   // the previous tile's epilogue reads of this warpgroup's staging rows are done
+      pipe_stage_acc<BN>(acc, acc_tile, wg);
+      named_bar_sync(1 + wg, 128);
+      epilogue_tile<BN, EPI>(g, acc_tile + wg * 64 * Cfg::ACC_PITCH, tid, b, mt * BM + wg * 64, nt * BN);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// 2-CTA variant (cta_group::2): a CTA pair (one cluster, one TPC) computes a 256 x BN tile.  Each CTA loads its own 128 A
-// rows and HALF of the W tile; the leader's single thread issues tcgen05.mma.cta_group::2 (M = 256) which reads both CTAs'
-// shared memory, so per-CTA smem/L2 traffic for W halves and the stages get deeper.  Barrier protocol:
-//   full[s]  (leader): 2 arrivals (each CTA's producer; the leader's carries expect_tx for BOTH CTAs' bytes); both CTAs'
-//                      TMA loads credit the leader's barrier (peer-bit-masked address)
-//   empty[s], tmem_full[a] (both CTAs): signalled by ONE multicast tcgen05.commit from the leader
-//   tmem_empty[a] (leader): 256 arrivals — the 128 epilogue threads of each CTA (the peer's arrive remotely)
-// ---------------------------------------------------------------------------------------------------------------
-template <int BN>
-struct Gemm2Cfg {
-  static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = (BN / 2) * BK * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BN >= 256) ? 6 : (BN >= 192) ? 7 : 8;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;
-  static constexpr int TMEM_COLS = (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-};
-
-template <int BN, int EPI>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm2_bf16_tc_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
-                     const GemmArgs g) {
-  using Cfg = Gemm2Cfg<BN>;
-  constexpr int STAGES = Cfg::STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-
-  __shared__ __align__(8) uint64_t full_bar[STAGES];
-  __shared__ __align__(8) uint64_t empty_bar[STAGES];
-  __shared__ __align__(8) uint64_t tmem_full_bar[2];
-  __shared__ __align__(8) uint64_t tmem_empty_bar[2];
-  __shared__ uint32_t tmem_base_slot;
-  __shared__ __align__(16) float epi_stage[EPI == PF_EPI_GATE_RESID ? 4 * 32 * EPI_PITCH : 4];
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tm_a);
-    tma_prefetch_desc(&tm_b);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full_bar[i], 2);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full_bar[i], 1);
-      mbar_init(&tmem_empty_bar[i], 256);
-    }
-    fence_barrier_init();
-  }
-  cluster_sync_all();          // barriers of both CTAs are initialised before anyone touches a remote one
-  if (warp == 2) {
-    tmem_alloc2(&tmem_base_slot, Cfg::TMEM_COLS);
-    tmem_relinquish2();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_slot;
-
-  const int num_kb = (g.k + BK - 1) / BK;
-  const int m2_tiles = (g.row_count + 2 * BM - 1) / (2 * BM);
-  const int tiles_per_batch = m2_tiles * g.n_tiles;
-  const int total_tiles = g.batches * tiles_per_batch;
-  const int cluster_id = blockIdx.x >> 1;
-  const int num_clusters = gridDim.x >> 1;
-
-  if (warp == 0 && elect_one()) {   // elect.sync: the compiler keeps the role's code on the uniform datapath
-    // ===== TMA producer (both CTAs) =====
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int tile = cluster_id; tile < total_tiles; tile += num_clusters) {
-      const int b = tile / tiles_per_batch;
-      const int r = tile - b * tiles_per_batch;
-      const int mt = r / g.n_tiles;
-      const int nt = r - mt * g.n_tiles;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-        if (leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * Cfg::STAGE_BYTES);
-        else mbar_arrive_remote(&full_bar[stage], 0);
-        tma_load_3d_2cta(sa, &tm_a, &full_bar[stage], kb * BK, g.row_begin + mt * 2 * BM + static_cast<int>(rank) * BM, b);
-        tma_load_2d_2cta(sa + Cfg::A_BYTES, &tm_b, &full_bar[stage], kb * BK, g.n_begin + nt * BN + static_cast<int>(rank) * (BN / 2));
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-  } else if (warp == 1 && leader && elect_one()) {
-    // ===== MMA issuer (leader CTA only) =====
-    constexpr uint32_t idesc = make_idesc_bf16(2 * BM, BN, 0, 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = cluster_id; tile < total_tiles; tile += num_clusters) {
-      mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + acc * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-        const uint64_t da = make_smem_desc_kmajor_sw128(sa);
-        const uint64_t db = make_smem_desc_kmajor_sw128(sa + Cfg::A_BYTES);
-#pragma unroll
-        for (int kk = 0; kk < BK / 16; ++kk)
-          umma_ss_2cta(tmem_d, da + 2 * kk, db + 2 * kk, idesc, (kb | kk) != 0 ? 1u : 0u);
-        umma_commit_2cta(&empty_bar[stage]);
-        if (kb == num_kb - 1) umma_commit_2cta(&tmem_full_bar[acc]);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue (both CTAs: each drains its own 128 rows from its own TMEM) =====
-    const int q = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = cluster_id; tile < total_tiles; tile += num_clusters) {
-      const int b = tile / tiles_per_batch;
-      const int r = tile - b * tiles_per_batch;
-      const int mt = r / g.n_tiles;
-      const int nt = r - mt * g.n_tiles;
-      const int m = mt * 2 * BM + static_cast<int>(rank) * BM + q * 32 + lane;
-      const int n_base = g.n_begin + nt * BN;
-      mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BN;
-      epilogue_tile<BN, EPI>(g, taddr, b, m, n_base, epi_stage + (EPI == PF_EPI_GATE_RESID ? q * 32 * EPI_PITCH : 0));
-      tc_fence_before();
-      if (leader) mbar_arrive(&tmem_empty_bar[acc]);
-      else mbar_arrive_remote(&tmem_empty_bar[acc], 0);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();          // nobody frees TMEM / exits while the peer may still reference this CTA's smem or barriers
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, Cfg::TMEM_COLS);
-  }
-}
-
-template <int BN, int EPI>
-static int launch_gemm2(const CUtensorMap& tm_a, const CUtensorMap& tm_b, const GemmArgs& g, cudaStream_t stream) {
-  using Cfg = Gemm2Cfg<BN>;
-  auto kern = gemm2_bf16_tc_kernel<BN, EPI>;
-  if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), Cfg::SMEM_BYTES, "gemm2")) return rc;
-  const int m2_tiles = (g.row_count + 2 * BM - 1) / (2 * BM);
-  const int total = g.batches * m2_tiles * g.n_tiles;
-  int sms = num_sms();
-  if (sms <= 0) sms = 148;
-  int clusters = sms / 2;
-  if (total < clusters) clusters = total;
-  kern<<<2 * clusters, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tm_a, tm_b, g);
-  return check_launch("pf_gemm_bf16(2cta)");
 }
 
 template <int BN, int EPI>
 static int launch_gemm(const CUtensorMap& tm_a, const CUtensorMap& tm_b, const GemmArgs& g, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
-  auto kern = gemm_bf16_tc_kernel<BN, EPI>;
+  using Cfg = PipeCfg<BN>;
+  auto kern = gemm_bf16_wgmma_kernel<BN, EPI>;
   if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), Cfg::SMEM_BYTES, "gemm")) return rc;
   const int total = g.batches * g.m_tiles * g.n_tiles;
   int grid = num_sms();
-  if (grid <= 0) grid = 148;
+  if (grid <= 0) grid = 132;
   if (total < grid) grid = total;
-  kern<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tm_a, tm_b, g);
+  kern<<<grid, PIPE_THREADS, Cfg::SMEM_BYTES, stream>>>(tm_a, tm_b, g);
   return check_launch("pf_gemm_bf16");
 }
 
 template <int EPI>
-static int dispatch_bn(int bn, const CUtensorMap& tm_a, const CUtensorMap& tm_b, const GemmArgs& g,
-                       cudaStream_t stream, bool two_cta) {
-  if (two_cta) {
-    switch (bn) {
-      case 256: return launch_gemm2<256, EPI>(tm_a, tm_b, g, stream);
-      case 192: return launch_gemm2<192, EPI>(tm_a, tm_b, g, stream);
-      case 128: return launch_gemm2<128, EPI>(tm_a, tm_b, g, stream);
-    }
-  }
+static int dispatch_bn(int bn, const CUtensorMap& tm_a, const CUtensorMap& tm_b, const GemmArgs& g, cudaStream_t stream) {
   switch (bn) {
-    case 256: return launch_gemm<256, EPI>(tm_a, tm_b, g, stream);
-    case 192: return launch_gemm<192, EPI>(tm_a, tm_b, g, stream);
     case 128: return launch_gemm<128, EPI>(tm_a, tm_b, g, stream);
     case 64: return launch_gemm<64, EPI>(tm_a, tm_b, g, stream);
   }
@@ -617,16 +327,8 @@ static int dispatch_bn(int bn, const CUtensorMap& tm_a, const CUtensorMap& tm_b,
 
 template <int EPI>
 static int warm_epi() {
-  int rc = 0;
-#define PF_WARM(KERN, CFG) if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(KERN), CFG::SMEM_BYTES, #KERN)
-  PF_WARM((gemm_bf16_tc_kernel<256, EPI>), GemmCfg<256>);
-  PF_WARM((gemm_bf16_tc_kernel<192, EPI>), GemmCfg<192>);
-  PF_WARM((gemm_bf16_tc_kernel<128, EPI>), GemmCfg<128>);
-  PF_WARM((gemm_bf16_tc_kernel<64, EPI>), GemmCfg<64>);
-  PF_WARM((gemm2_bf16_tc_kernel<256, EPI>), Gemm2Cfg<256>);
-  PF_WARM((gemm2_bf16_tc_kernel<192, EPI>), Gemm2Cfg<192>);
-  PF_WARM((gemm2_bf16_tc_kernel<128, EPI>), Gemm2Cfg<128>);
-#undef PF_WARM
+  int rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_bf16_wgmma_kernel<128, EPI>), PipeCfg<128>::SMEM_BYTES, "gemm<128>");
+  if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_bf16_wgmma_kernel<64, EPI>), PipeCfg<64>::SMEM_BYTES, "gemm<64>");
   return rc;
 }
 // load every instantiation and set its dynamic-smem attribute on the current device (so nothing initialises inside a
@@ -659,10 +361,9 @@ extern "C" int pf_gemm_bf16(const pf_gemm_desc* d, void* stream_) {
   const int epi = d->epilogue;
   PF_REQUIRE(epi >= 0 && epi <= PF_EPI_QKV_GELU, "pf_gemm_bf16: unknown epilogue %d", epi);
 
-  // Column tiling: 256-wide tiles wherever they fit (and a 128-wide tail launch when n = 256 a + 128, e.g. 1920 / 5760),
-  // otherwise the widest of 192 / 128 / 64 that divides n.  The QKV epilogues work per 64-column head, so any multiple of 64
-  // is head-aligned.
-  int bn = 0, n_main = d->n, bn_tail = 0;
+  // Column tiling: 128-wide tiles (64 x 128 fp32 accumulators per consumer warpgroup) when they divide n, else 64-wide.  The QKV
+  // epilogues work per 64-column head, so any multiple of 64 is head-aligned.
+  int bn = 0;
   const bool qkv = (epi == PF_EPI_QKV_ROPE || epi == PF_EPI_QKV_GELU);
   if (qkv) {
     PF_REQUIRE(d->head_dim == 64, "pf_gemm_bf16: QKV epilogue supports head_dim 64 only (got %d)", d->head_dim);
@@ -685,22 +386,8 @@ extern "C" int pf_gemm_bf16(const pf_gemm_desc* d, void* stream_) {
                "pf_gemm_bf16: output must be 16-byte aligned (ldo %lld col %d)", (long long)d->ldo, d->out_col_begin);
   }
   PF_REQUIRE(d->n % 64 == 0, "pf_gemm_bf16: n=%d must be a multiple of 64", d->n);
-  if (epi == PF_EPI_QKV_GELU) {
-    // tiles must not straddle the q|k|v / mlp boundary (different epilogue per tile): keep the uniform 192/128/64 tiling
-    bn = (d->n_split % 192 == 0 && d->n % 192 == 0) ? 192 : ((d->n_split % 128 == 0 && d->n % 128 == 0) ? 128 : 64);
-  } else if (d->n % 256 == 0) {
-    bn = 256;
-  } else if (d->n % 256 == 128 && d->n > 256) {
-    bn = 256;
-    n_main = d->n - 128;
-    bn_tail = 128;
-  } else if (d->n % 192 == 0) {
-    bn = 192;
-  } else if (d->n % 128 == 0) {
-    bn = 128;
-  } else {
-    bn = 64;
-  }
+  // QKV_GELU: tiles must not straddle the q|k|v / mlp boundary (different epilogue per tile)
+  bn = (d->n % 128 == 0 && (epi != PF_EPI_QKV_GELU || d->n_split % 128 == 0)) ? 128 : 64;
 
   GemmArgs g{};
   g.batches = d->batches;
@@ -742,52 +429,24 @@ extern "C" int pf_gemm_bf16(const pf_gemm_desc* d, void* stream_) {
     for (int i = 0; i < d->peer_count; ++i) PF_REQUIRE(d->peer_qkv[i] != nullptr, "pf_gemm_bf16: peer_qkv[%d] is null", i);
   }
 
-  // 2-CTA tiles (256 x BN, cta_group::2) pay off for 256-wide tiles and for short-K 192-wide ones (measured A/B on
-  // B200: +11 % at N=7680/K=1920, -1..3 % at N=1920/K>=7680); kernel_variant 1/2 pins the 1-CTA / 2-CTA kernel
+  // kernel_variant 1 / 2 pins the 128-wide / 64-wide tile kernel
   PF_REQUIRE(d->kernel_variant >= 0 && d->kernel_variant <= 2, "pf_gemm_bf16: bad kernel_variant %d", d->kernel_variant);
-  const int env_2cta = d->kernel_variant == 1 ? 0 : d->kernel_variant == 2 ? 1 : -1;
-  auto want_2cta = [&](int tile_n) {
-    bool t = d->row_count >= 1024 && (tile_n == 256 || (tile_n == 192 && d->k <= 2048));
-    if (env_2cta == 0) t = false;
-    if (env_2cta == 1 && tile_n >= 128) t = true;
-    return t;
-  };
-  // Wave quantisation: with few rows (a sequence-parallel rank's chunk) the 256-wide tiling leaves the last wave of the
-  // persistent grid mostly idle (M=3872, N=1920: 112 tile pairs on 74 SM pairs = 2 waves for 1.5 waves of work, plus a
-  // 128-wide tail launch).  A narrower tiling changes neither the K order nor the bits, so pick the one whose wave count x
-  // tile cost is smallest (tile efficiencies measured on B200: 256 -> 1.0, 192 -> 0.97, 128 -> 0.90).
-  if (epi != PF_EPI_QKV_GELU && d->kernel_variant == 0 && get_option(PF_OPT_GEMM_WAVE_TILING)) {
+  PF_REQUIRE(d->kernel_variant != 1 || bn == 128, "pf_gemm_bf16: kernel_variant 1 (128-wide tiles) needs n %% 128 == 0");
+  if (d->kernel_variant == 2) bn = 64;
+  // Wave quantisation: with few rows (a sequence-parallel rank's chunk) the last wave of the persistent grid can be mostly
+  // idle.  The 64-wide tiling changes neither the K order nor the bits, so take it when its waves x tile width, over the
+  // 64-wide kernel's efficiency, is smaller.  Efficiency 0.75 of the 128-wide kernel: measured on an H100 80GB HBM3 (700 W) at
+  // M = 30976, K = 1920 / 7680, N = 1920 / 7680, where the same GEMMs took 1.33 - 1.37 x as long with 64-wide tiles
+  // (bench.py per-family breakdown, e.g. ff2 15.2 -> 20.5 ms, single_out 34.2 -> 46.9 ms).
+  if (bn == 128 && d->kernel_variant == 0 && get_option(PF_OPT_GEMM_WAVE_TILING)) {
     int sms = num_sms();
-    if (sms <= 0) sms = 148;
-    auto part_cost = [&](int tile_n, int ncols) -> double {
-      const bool two = want_2cta(tile_n);
-      const long long mt = (d->row_count + (two ? 2 * BM : BM) - 1) / (two ? 2 * BM : BM);
-      const long long tiles = static_cast<long long>(d->batches) * mt * (ncols / tile_n);
-      const long long units = two ? sms / 2 : sms;
-      const long long waves = (tiles + units - 1) / units;
-      const double eff = tile_n == 256 ? 1.0 : tile_n == 192 ? 0.97 : tile_n == 128 ? 0.90 : 0.75;
-      return static_cast<double>(waves) * tile_n / eff;
+    if (sms <= 0) sms = 132;
+    auto cost = [&](int tile_n) -> double {
+      const long long tiles = static_cast<long long>(d->batches) * ((d->row_count + BM - 1) / BM) * (d->n / tile_n);
+      const long long waves = (tiles + sms - 1) / sms;
+      return static_cast<double>(waves) * tile_n / (tile_n == 128 ? 1.0 : 0.75);
     };
-    const double cur = part_cost(bn, n_main) + (bn_tail ? part_cost(bn_tail, d->n - n_main) : 0.0);
-    const double ideal = static_cast<double>(d->batches) * d->row_count * d->n / (static_cast<double>(sms) * BM);
-    if (cur > 1.15 * ideal) {          // only where the quantisation loss is material
-      int best_bn = bn, best_tail = bn_tail, best_main = n_main;
-      double best = cur;
-      const int cands[2] = {192, 128};
-      for (int c : cands) {
-        if (d->n % c != 0 || c >= bn) continue;
-        const double cc = part_cost(c, d->n);
-        if (cc < 0.95 * best) {
-          best = cc;
-          best_bn = c;
-          best_tail = 0;
-          best_main = d->n;
-        }
-      }
-      bn = best_bn;
-      bn_tail = best_tail;
-      n_main = best_main;
-    }
+    if (cost(64) < cost(128)) bn = 64;
   }
   CUtensorMap tm_a;
   {
@@ -801,29 +460,23 @@ extern "C" int pf_gemm_bf16(const pf_gemm_desc* d, void* stream_) {
     if (rc) return rc;
   }
 
-  auto launch_part = [&](int tile_n, int n_begin, int n_count) -> int {
-    const bool two_cta = want_2cta(tile_n);
-    CUtensorMap tm_b;
+  CUtensorMap tm_b;
+  {
     const uint64_t dims[2] = {static_cast<uint64_t>(d->k), static_cast<uint64_t>(d->n)};
     const uint64_t strides[1] = {static_cast<uint64_t>(d->k) * 2};
-    const uint32_t box[2] = {BK, static_cast<uint32_t>(two_cta ? tile_n / 2 : tile_n)};
+    const uint32_t box[2] = {BK, static_cast<uint32_t>(bn)};
     int rc = encode_tensor_map(&tm_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, d->w, dims, strides, box,
                                CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
-    GemmArgs gp = g;
-    gp.n_begin = n_begin;
-    gp.n_tiles = n_count / tile_n;
-    switch (epi) {
-      case PF_EPI_STORE_BF16: return dispatch_bn<PF_EPI_STORE_BF16>(tile_n, tm_a, tm_b, gp, stream, two_cta);
-      case PF_EPI_GELU_BF16: return dispatch_bn<PF_EPI_GELU_BF16>(tile_n, tm_a, tm_b, gp, stream, two_cta);
-      case PF_EPI_STORE_F32: return dispatch_bn<PF_EPI_STORE_F32>(tile_n, tm_a, tm_b, gp, stream, two_cta);
-      case PF_EPI_GATE_RESID: return dispatch_bn<PF_EPI_GATE_RESID>(tile_n, tm_a, tm_b, gp, stream, two_cta);
-      case PF_EPI_QKV_ROPE: return dispatch_bn<PF_EPI_QKV_ROPE>(tile_n, tm_a, tm_b, gp, stream, two_cta);
-      case PF_EPI_QKV_GELU: return dispatch_bn<PF_EPI_QKV_GELU>(tile_n, tm_a, tm_b, gp, stream, two_cta);
-    }
-    return -1;
-  };
-  int rc = launch_part(bn, 0, n_main);
-  if (rc == 0 && bn_tail) rc = launch_part(bn_tail, n_main, d->n - n_main);
-  return rc;
+  }
+  g.n_tiles = d->n / bn;
+  switch (epi) {
+    case PF_EPI_STORE_BF16: return dispatch_bn<PF_EPI_STORE_BF16>(bn, tm_a, tm_b, g, stream);
+    case PF_EPI_GELU_BF16: return dispatch_bn<PF_EPI_GELU_BF16>(bn, tm_a, tm_b, g, stream);
+    case PF_EPI_STORE_F32: return dispatch_bn<PF_EPI_STORE_F32>(bn, tm_a, tm_b, g, stream);
+    case PF_EPI_GATE_RESID: return dispatch_bn<PF_EPI_GATE_RESID>(bn, tm_a, tm_b, g, stream);
+    case PF_EPI_QKV_ROPE: return dispatch_bn<PF_EPI_QKV_ROPE>(bn, tm_a, tm_b, g, stream);
+    case PF_EPI_QKV_GELU: return dispatch_bn<PF_EPI_QKV_GELU>(bn, tm_a, tm_b, g, stream);
+  }
+  return -1;
 }

@@ -5,7 +5,7 @@ Mirrors the call surface `PyramidDiTForVideoGeneration` uses (pyramid_dit/pyrami
     dit(sample=[clips], timestep_ratio=t, encoder_hidden_states=e, encoder_attention_mask=m, pooled_projections=p)[0]
 
 plus `.config.in_channels`, `.parameters()`, `.device`, `.dtype`, `.to()`; weights are imported from a state-dict in the
-reference key layout (SURVEY.md §8b).  The forward is a fixed sequence of libpf_b200 kernel launches on the current CUDA
+reference key layout.  The forward is a fixed sequence of libpf_b200 kernel launches on the current CUDA
 stream (no torch math on the path, no CPU fallback):
 
   conditioning GEMVs -> all-layer AdaLN modulation GEMV -> embedders (GEMM, fp32 store into the joint residual stream)
@@ -100,7 +100,7 @@ class SeqPlan:
     seg: torch.Tensor         # device int32 [B, S]
     time: torch.Tensor        # device int32 [B, S]
     sched: torch.Tensor       # device int32 [B, q_tiles, stride]
-    sched2: object            # ops.PairSchedule on the device: pair schedule + row masks of the two-q-tile attention kernel
+    sched2: object            # ops.PairSchedule on the device: pair schedule + row masks (pf_attn_build_pair_*)
     allowed_pairs: int        # sum over batch of allowed (q, kv) pairs (attention FLOP accounting)
 
 
@@ -201,7 +201,7 @@ class B200FluxTransformer(torch.nn.Module):
         # does not depend on how fast the host can walk the launch sequence (ctypes + descriptor encoding per launch).
         # Off by default: callers that reuse shapes for many steps (sampler, bench) turn it on.
         self.trim_last_block = True     # last single block on the current clip's rows only (exact; see forward)
-        self.attn_variant = 0           # pf_attn_desc.variant (0 = the default two-q-tile kernel); bench/tests A/B others
+        self.attn_variant = 0           # pf_attn_desc.variant (every value runs the one sm_90a kernel)
         self.use_cuda_graph = False
         self._graphs: "Dict[tuple, dict]" = {}
         self._graph_warm = False
@@ -221,7 +221,7 @@ class B200FluxTransformer(torch.nn.Module):
                              axes_dims_rope=tuple(rc.axes_dims_rope))
         return cls(cfg, ref_module.state_dict(), device=device, **kw)
 
-    # -- weight import (reference key layout, SURVEY.md §8b) -----------------------------------------------------------
+    # -- weight import (reference key layout) ---------------------------------------------------------------------------
     def _import_state_dict(self, sd: Dict[str, torch.Tensor], device) -> None:
         c = self.cfg
         d = c.inner_dim
@@ -401,8 +401,7 @@ class B200FluxTransformer(torch.nn.Module):
         assert len(sample) == 1, "inference passes one stage per call (pipeline P:760-766)"
         clips = sample[0] if isinstance(sample[0], (list, tuple)) else [sample[0]]
         lay = getattr(self, "layout", None)
-        # the NCCL formulation of the parallel step stays host-launched (capturing its all-to-alls hung on the 2-GPU box in
-        # round 1); the peer-memory formulation is plain kernels and is captured like the single-GPU step
+        # the NCCL formulation of the parallel step stays host-launched (its all-to-alls are not captured); the peer-memory formulation is plain kernels and is captured like the single-GPU step
         nccl_par = lay is not None and lay.enabled and getattr(self, "exchange", DEFAULT_EXCHANGE) == "nccl"
         if self.use_cuda_graph and not nccl_par and not self.timer.enabled and self.attn_events is None:
             return self._forward_graphed(list(clips), timestep_ratio, encoder_hidden_states, encoder_attention_mask,
@@ -693,7 +692,7 @@ class B200FluxTransformer(torch.nn.Module):
             out = full
         return [out]
 
-    # accounting used by bench.py / DESIGN.md (SURVEY.md §8d "algorithmic work per unit")
+    # accounting used by bench.py / DESIGN.md (algorithmic work per unit)
     def step_flops(self, b: int, plan: SeqPlan) -> Dict[str, float]:
         c = self.cfg
         d = c.inner_dim

@@ -1,7 +1,7 @@
 """B200MMDiT — drop-in for the reference `PyramidDiffusionMMDiT` (SD3 variant) on the sampler hot path.
 
 Same call surface as `B200FluxTransformer` (pipeline P:760-766); weights from the reference state-dict key layout
-(`pos_embed.{pos_embed,proj}`, `attn.norm_add_q/k`, last block without `to_add_out` / `ff_context`; SURVEY.md §8b).
+(`pos_embed.{pos_embed,proj}`, `attn.norm_add_q/k`, last block without `to_add_out` / `ff_context`).
 Reuses the miniFLUX kernels unchanged — 24 double blocks at D=1536 / 24 heads — with three host-side differences:
   * patch embed = conv2d(k=2, s=2) (mmdit_modules/modeling_embedding.py:231) run as the patchify + GEMM pair with the conv
     weight re-ordered to the (p1 p2 c) feature order; the cropped / bilinearly down-sampled 2-D sincos table

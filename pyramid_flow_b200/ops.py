@@ -10,7 +10,7 @@ from typing import Optional
 import torch
 
 from . import _lib
-from ._lib import (AttnDesc, GemmDesc, UmmaProbe, PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_GELU,
+from ._lib import (AttnDesc, GemmDesc, PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_GELU,
                    PF_EPI_QKV_ROPE, PF_EPI_STORE_BF16, PF_EPI_STORE_F32)
 
 
@@ -163,10 +163,10 @@ def attn_build_schedule(seg: torch.Tensor, time: torch.Tensor):
 
 
 class PairSchedule:
-    """Schedule of the two-q-tile attention kernel: `sched` int32 [batch, n_pairs, stride] (pf_attn_build_pair_schedule),
+    """Schedule of pairs of q tiles: `sched` int32 [batch, n_pairs, stride] (pf_attn_build_pair_schedule),
     `mask_index` int32 [batch, n_pairs, 2 * stride] and `mask_bits` int32 [blocks, 128, 4] (pf_attn_build_pair_masks).
     `group3` (optional) = the same three tensors for groups of three q tiles (pf_attn_build_group_schedule / _masks), the
-    schedule of the three-q-tile kernel."""
+    schedule of groups of three q tiles."""
 
     def __init__(self, sched: torch.Tensor, mask_index: torch.Tensor, mask_bits: torch.Tensor,
                  group3: Optional["PairSchedule"] = None):
@@ -186,8 +186,8 @@ class PairSchedule:
 
 
 def attn_build_pair_schedule(sched: torch.Tensor, seq: int, seg: torch.Tensor, time: torch.Tensor) -> PairSchedule:
-    """Tile schedule (int32 CPU [batch, q_tiles, stride]) + the seg/time ids -> PairSchedule (CPU tensors) of the two-q-tile
-    kernel: merged kv lists of adjacent q tiles and the precomputed 128-bit row masks of their partial tiles."""
+    """Tile schedule (int32 CPU [batch, q_tiles, stride]) + the seg/time ids -> PairSchedule (CPU tensors) of the q-tile pairs:
+    merged kv lists of adjacent q tiles and the precomputed 128-bit row masks of their partial tiles."""
     sched = sched.to(torch.int32).contiguous().cpu()
     seg = seg.to(torch.int32).contiguous().cpu()
     time = time.to(torch.int32).contiguous().cpu()
@@ -211,7 +211,7 @@ def attn_build_pair_schedule(sched: torch.Tensor, seq: int, seg: torch.Tensor, t
 
 def attn_build_group_schedule(sched: torch.Tensor, seq: int, seg: torch.Tensor, time: torch.Tensor, group: int = 3,
                               share: Optional[PairSchedule] = None) -> PairSchedule:
-    """The pair schedule generalised to groups of `group` q tiles (the three-q-tile kernel): sched int32 [batch, n_groups,
+    """The pair schedule generalised to groups of `group` q tiles: sched int32 [batch, n_groups,
     stride] with entries (kv_tile << 8) | 2 flag bits per tile, mask_index [batch, n_groups, group * stride], mask_bits.
     `share` = the pair schedule of the same tile schedule: its block pool is reused (a block depends on (q tile, kv tile) only),
     no bits are built and `mask_bits` IS `share.mask_bits`."""
@@ -279,19 +279,3 @@ def attn_fwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tenso
             assert g3.sched.shape[-1] == sched.shape[-1]
             d.group_sched, d.group_mask_index, d.group_mask_bits = g3.sched.data_ptr(), g3.mask_index.data_ptr(), g3.mask_bits.data_ptr()
     _lib.check(_lib.load().pf_attn_fwd_masked(C.byref(d), _lib.stream_ptr()), "pf_attn_fwd_masked")
-
-
-def debug_umma(a: torch.Tensor, b: torch.Tensor, n: int, k: int, *, b_box_rows: int, b_mn_major: int, b_lbo: int,
-               b_sbo: int, b_k_step_bytes: int, b_kblock_bytes: int, a_from_tmem: int, a_row_offset: int = 0,
-               a_base_offset: int = 0) -> torch.Tensor:
-    d = torch.zeros(128, n, dtype=torch.float32, device=a.device)
-    p = UmmaProbe()
-    p.a, p.b, p.d = a.data_ptr(), b.data_ptr(), d.data_ptr()
-    p.n, p.k = n, k
-    p.b_rows, p.b_cols = b.shape
-    p.b_box_rows, p.b_mn_major = b_box_rows, b_mn_major
-    p.b_lbo, p.b_sbo, p.b_k_step_bytes, p.b_kblock_bytes = b_lbo, b_sbo, b_k_step_bytes, b_kblock_bytes
-    p.a_rows, p.a_row_offset, p.a_base_offset = a.shape[0], a_row_offset, a_base_offset
-    p.a_from_tmem = a_from_tmem
-    _lib.check(_lib.load().pf_debug_umma(C.byref(p), _lib.stream_ptr()), "pf_debug_umma")
-    return d

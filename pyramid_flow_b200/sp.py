@@ -2,7 +2,7 @@
 
 Follows the reference's sequence-parallel layout (trainer_misc/sp_utils.py:21-47 groups; Ulysses-style head<->sequence
 all-to-all at the attention boundary, flux_modules/modeling_flux_block.py:266-325, 519-565 via trainer_misc/communicate.py)
-with two changes the reference cannot make (SURVEY.md §5, §8e):
+with two changes the reference cannot make:
   * the CFG pair is split first (uncond / cond on separate halves of the world: no traffic until the velocity combine),
     so every rank runs batch 1 and the reference's `B % sp == 0` transposition trick (F:471-485) is not needed;
   * 30 heads do not divide by 4 or 8: heads are zero-padded to the next multiple of the SP degree (32 at sp=4, a 6.7 %

@@ -6,12 +6,12 @@ Call surface used by the pipeline (pyramid_dit_for_video_gen_pipeline.py:1221-12
     self.vae.encode(image[:, :, None]).latent_dist.sample()                                        # i2v image latent
 
 plus `.device`, `.dtype`, `.to()`, `.enable_tiling()`.  Weights come from a state-dict in the reference key layout
-(`decoder.*`, `post_quant_conv.*`, and — when present — `encoder.*`, `quant_conv.*`; SURVEY.md §8b).  The encoder reuses the
+(`decoder.*`, `post_quant_conv.*`, and — when present — `encoder.*`, `quant_conv.*`).  The encoder reuses the
 decoder's kernels; its down-samplers are the same implicit-GEMM conv with a strided TMA box (`stride_*` in pf_conv3d_desc).
 
 Execution model (all math in libpf_b200 kernels, channels-last bf16 activations `[T, H, W, C]`, batch handled one sample
 at a time as the pipeline does):
-  * every CausalConv3d  -> `pf_causal_conv3d` (tcgen05 implicit GEMM, TMA im2col-free, bias/residual/depth-to-space fused)
+  * every CausalConv3d  -> `pf_causal_conv3d` (wgmma implicit GEMM, TMA im2col-free, bias/residual/depth-to-space fused)
   * every CausalGroupNorm(+SiLU) -> `pf_groupnorm_stats` + `pf_groupnorm_apply`, the apply writing straight into the next
     conv's input buffer behind its 2-frame causal halo
   * mid-block attention -> 1x1x1 convs for q/k/out, `pf_gemm_bf16` for V^T, QK^T and PV, `pf_softmax_rows`

@@ -8,21 +8,9 @@ sys.path.insert(0, str(ROOT))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu)")
 
 
 @pytest.fixture(scope="session")
 def golden_dir():
     return ROOT / "tests" / "golden"
-
-
-@pytest.fixture(scope="session", autouse=True)
-def _library_options_from_env():
-    """PF_TEST_ATTN_TRIPLE=0 / 1 runs the whole suite with the two-q-tile / three-q-tile attention kernel as the default one
-    (unset: the library default, the three-q-tile kernel)."""
-    import os
-    v = os.environ.get("PF_TEST_ATTN_TRIPLE")
-    if v in ("0", "1"):
-        from pyramid_flow_b200 import _lib
-        _lib.set_option(_lib.PF_OPT_ATTN_TRIPLE_KERNEL, int(v))
-    yield

@@ -1,7 +1,7 @@
-"""Every conv kernel the VAE number rests on, pinned one by one through pf_conv3d_desc.kernel_variant (1 = conv3d 1-CTA,
-2 = conv3d2 2-CTA pairs, 3 = conv3d2w 2-CTA with kw-tap reuse) at shapes with >= 3 tiles along W (halo reuse across W tiles),
+"""Every conv kernel the VAE number rests on, pinned one by one through pf_conv3d_desc.kernel_variant (1 = 128-wide filter
+tiles, 2 = 64-wide filter tiles) at shapes with >= 3 tiles along W (halo reuse across W tiles),
 ragged last tiles, and at the headline layer shapes (128->128 @768x1280, 256->256 @384x640: sampled voxels vs fp32);
-plus the full-resolution (96x160 latent) VAE decode against the fp32 oracle on the same GPU.  Needs a B200."""
+plus the full-resolution (96x160 latent) VAE decode against the fp32 oracle on the same GPU.  Needs an H100."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -49,7 +49,7 @@ def _sampled_err(x, wt, bias, out, n=8192):
 
 @pytest.mark.parametrize("ci,co,t,h,w", [(64, 128, 2, 5, 300), (128, 256, 3, 4, 417), (128, 128, 2, 12, 1280), (256, 512, 1, 7, 384)])
 def test_conv_kernel_variants_multi_tile_w(ci, co, t, h, w):
-    """>= 3 (up to 10) 128-voxel tiles along W, ragged last tile: every kernel vs F.conv3d, and all three kernels give the
+    """>= 3 (up to 10) 128-voxel tiles along W, ragged last tile: every kernel vs F.conv3d, and both kernels give the
     SAME BITS (one K accumulation order), so the dispatch never changes results."""
     dev = torch.device("cuda:0")
     cv, wt, bias = _mk(ci, co, dev, seed=ci + w)
@@ -60,27 +60,27 @@ def test_conv_kernel_variants_multi_tile_w(ci, co, t, h, w):
     xr = F.pad(x.permute(3, 0, 1, 2)[None].float(), (1, 1, 1, 1, 2, 0))
     ref = F.conv3d(xr, wt, bias)[0].permute(1, 2, 3, 0)
     outs = {}
-    for variant in (1, 2, 3):
+    for variant in (1, 2):
         outs[variant] = _run(cv, xin, t, h, w, co, variant)
         err = (outs[variant].float() - ref).abs().max().item()
         assert err < 3e-2, (variant, ci, co, w, err)
-    assert torch.equal(outs[1], outs[2]) and torch.equal(outs[2], outs[3]), "kernel variants must agree bit for bit"
+    assert torch.equal(outs[1], outs[2]), "kernel variants must agree bit for bit"
     auto = _run(cv, xin, t, h, w, co, 0)
     assert torch.equal(auto, outs[1])
-    # residual + store into a haloed buffer through the kw-reuse kernel
+    # residual + store into a haloed buffer
     res = torch.randn(t, h, w, co, device=dev).bfloat16()
     from pyramid_flow_b200.vae import B200CausalVAE
     holder = B200CausalVAE.__new__(B200CausalVAE)
     out2 = torch.zeros(t + 2, h, w, co, device=dev, dtype=torch.bfloat16)
-    B200CausalVAE._conv(holder, cv, xin, t, h, w, out=out2, out_t_offset=2, residual=res, kernel_variant=3)
+    B200CausalVAE._conv(holder, cv, xin, t, h, w, out=out2, out_t_offset=2, residual=res, kernel_variant=2)
     torch.cuda.synchronize()
     assert (out2[2:].float() - (ref + res.float())).abs().max().item() < 4e-2 and bool((out2[:2] == 0).all())
 
 
 @pytest.mark.parametrize("ci,co,t,h,w", [(128, 128, 2, 768, 1280), (256, 256, 2, 384, 640)])
 def test_conv_headline_layer_shapes(ci, co, t, h, w):
-    """The layers the decode time is made of (up3 128->128 at 768x1280, up2 256->256 at 384x640): the default dispatch (kw-reuse
-    2-CTA kernel) and the per-tap 2-CTA kernel, verified on 8192 sampled voxels (borders and W-tile seams included) in fp32."""
+    """The layers the decode time is made of (up3 128->128 at 768x1280, up2 256->256 at 384x640): the default dispatch
+    and the 64-wide-tile kernel, verified on 8192 sampled voxels (borders and W-tile seams included) in fp32."""
     dev = torch.device("cuda:0")
     cv, wt, bias = _mk(ci, co, dev, seed=7)
     torch.manual_seed(3)
@@ -123,5 +123,5 @@ def test_vae_decode_full_resolution_matches_oracle():
     print(f"VAE 96x160 latent -> {tuple(out.shape)}: ours vs fp32 oracle max_abs {err:.3e} mse {mse:.3e} | reference bf16 policy "
           f"max_abs {e2:.3e} mse {m2:.3e} | |ref| mean {ref.abs().mean():.3f}")
     assert out.shape == ref.shape == (1, 3, 17, 768, 1280)
-    assert err < 8.8e-2 and mse < 7.3e-5               # measured 6.70e-2 / 5.61e-5 (max over 5e7 values) x 1.3
+    assert err < 8.8e-2 and mse < 7.3e-5
     assert mse <= 2.0 * m2 + 1e-5, "must be comparable to the reference's own bf16 error"

@@ -1,4 +1,4 @@
-"""Parity of the CUDA DiT step (through the C-ABI) against the oracle / the reference's golden outputs. Needs a B200."""
+"""Parity of the CUDA DiT step (through the C-ABI) against the oracle / the reference's golden outputs. Needs an H100."""
 import pytest
 import torch
 
@@ -8,7 +8,7 @@ pytestmark = pytest.mark.gpu
 # Velocities are O(1) (|v| mean ~0.9 for the synthetic weights); all GEMM/attention operands are bf16 (ulp(1) = 7.8e-3),
 # accumulation, LN/RMS statistics, softmax and the residual stream are fp32.  Measured error is reported next to the
 # error of the reference's own dtype policy (oracle under bf16 autocast) against the same fp32 truth.
-# Measured on B200 (round 2): 9.1e-3 .. 1.17e-2 max-abs, 4.2e-6 .. 4.4e-6 mse over the cases below; thresholds = max x 1.3.
+# Thresholds = 1.3 x the error of the first implementation of these kernels; the sm_90a kernels are held to the same ones.
 TOL_MAX_ABS = 1.5e-2
 TOL_MSE = 6e-6
 

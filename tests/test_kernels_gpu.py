@@ -1,4 +1,4 @@
-"""Per-kernel parity through the C-ABI on B200 (ragged shapes included): GEMM epilogues, attention mask cases,
+"""Per-kernel parity through the C-ABI on an H100 (ragged shapes included): GEMM epilogues, attention mask cases,
 elementwise kernels.  The checker for a single floating-point kernel is a plain PyTorch fp32 reference of the same op."""
 import pytest
 import os
@@ -97,8 +97,8 @@ def test_gemm_epilogues_row_ranges():
     assert _rel(cat[..., D:], F.gelu(x.float() @ wm.float().t() + bm, approximate="tanh")) < 8e-3
 
 
-# pf_attn_desc.variant: 3 = one-q-tile kernel (round 1, kept for A/B), 0x10 = two-q-tile kernel, 0x20 = three-q-tile kernel, 0 =
-# default (= 0x20 when the schedules are given; 0x10 for launches with peer stores)
+# pf_attn_desc.variant: every accepted value (3, 0x10 with the pair schedule, 0x20 with the group schedule, 0 = default) must
+# give the same, correct result; the sm_90a library runs one kernel for all of them
 # PF_TEST_ATTN_EXTRA = further variant codes to put through the same cases
 ATTN_EXTRA = [int(x, 0) for x in os.environ.get("PF_TEST_ATTN_EXTRA", "").split()]
 ATTN_VARIANTS = [3, 0x10, 0x20, 0] + ATTN_EXTRA
@@ -194,8 +194,7 @@ def test_attention_adversarial_score_jumps():
             assert own == sched[0, t, 1:1 + int(sched[0, t, 0])].tolist()
     sg, tm = seg.to(DEV), tim.to(DEV)
     ref, _ = _attn_ref(q, k, v, sg, tm)
-    # the one-tile kernel (variant 3) exponentiates against a max that is one tile stale and is NOT safe on such inputs (it
-    # is kept for A/B timing only); the two-q-tile kernel has an exact per-row max and must be exact here
+    # the online softmax keeps an exact per-row running max and must be exact on such inputs
     for variant in [0x10, 0x20, 0] + ATTN_EXTRA:
         out = torch.zeros(B, S, H * 64, device=DEV, dtype=torch.bfloat16)
         ops.attn_fwd(q, k, v, out, sg, tm, sched.to(DEV), 0.125, variant=variant, pair_sched=pso.to(DEV))

@@ -1,10 +1,10 @@
-"""Parity of the CUDA SD3-MMDiT step (BASELINE configs[4] path) against the reference golden / oracle. Needs a B200."""
+"""Parity of the CUDA SD3-MMDiT step (BASELINE configs[4] path) against the reference golden / oracle. Needs an H100."""
 import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
-TOL_MAX_ABS = 1.55e-2  # measured 8.6e-3 .. 1.195e-2 (round 2) x 1.3
-TOL_MSE = 6e-6         # measured 4.0e-6 .. 4.4e-6
+TOL_MAX_ABS = 1.55e-2
+TOL_MSE = 6e-6
 
 
 def _run(cfg_kw, params, clips, t, enc, mask, pooled):

@@ -136,7 +136,7 @@ def test_c_abi_rejects_bad_arguments_with_a_message():
 
 
 def test_pair_schedule_is_the_union_of_the_two_tile_rows():
-    """pf_attn_build_pair_schedule (host code of the two-q-tile attention kernel): pair p = q tiles (q_tiles-2-2p, q_tiles-1-2p);
+    """pf_attn_build_pair_schedule (host code): pair p = q tiles (q_tiles-2-2p, q_tiles-1-2p);
     its row is the sorted union of the two tiles' kv lists; per-tile flags reproduce each tile's own list and mask bits; a
     missing lower tile (odd q_tiles) contributes nothing."""
     import torch
@@ -184,7 +184,7 @@ def test_pair_schedule_is_the_union_of_the_two_tile_rows():
 
 
 def test_group_schedule_is_the_union_of_the_three_tile_rows():
-    """pf_attn_build_group_schedule / _masks (host code of the opt-in three-q-tile attention kernel): group g = q tiles
+    """pf_attn_build_group_schedule / _masks (host code): group g = q tiles
     q_tiles-3-3g .. q_tiles-1-3g; its row is the sorted union of the tiles' kv lists, per-tile flags reproduce each tile's own
     list, missing leading tiles contribute nothing, and the row masks equal the dense mask definition (F:318-350)."""
     import torch

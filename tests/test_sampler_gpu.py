@@ -1,4 +1,4 @@
-"""Loop-level parity on B200: the sampler mirror driving the CUDA DiT vs the same loop driving the fp32 oracle
+"""Loop-level parity on an H100: the sampler mirror driving the CUDA DiT vs the same loop driving the fp32 oracle
 (identical start noise, injected block noise and text embeddings) -> final-latent error (BASELINE.json north_star)."""
 import pytest
 import torch

@@ -23,7 +23,7 @@ def test_scheduler_tables_match_reference(golden_dir):
             # what the DiT actually sees is the bf16-rounded timestep (pipeline P:750): identical
             assert torch.equal(s.timesteps.bfloat16(), g[f"timesteps_{n}_{st}"].bfloat16())
             assert torch.equal(s.sigmas, g[f"sigmas_{n}_{st}"])
-    # published stage boundaries (SURVEY.md a14): start sigmas {1.0, 0.80024, 0.50075}, end {0.667, 0.334, 0}
+    # published stage boundaries start sigmas {1.0, 0.80024, 0.50075}, end {0.667, 0.334, 0}
     assert abs(s.start_sigmas[1] - 0.80024) < 1e-5 and abs(s.start_sigmas[2] - 0.50075) < 1e-5
 
 

@@ -1,4 +1,4 @@
-"""Parity of the CUDA causal-VAE decode (through the C-ABI) against the oracle / the reference's golden output. B200."""
+"""Parity of the CUDA causal-VAE decode (through the C-ABI) against the oracle / the reference's golden output. Needs an H100."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -8,7 +8,7 @@ pytestmark = pytest.mark.gpu
 # bf16 activations through ~60 convs + 30 GroupNorms; decoded samples are O(0.5) (|ref| mean ~0.43, range ~[-2, 2]).
 # Stated tolerance on the decoded sample vs the fp32 oracle: max-abs 0.1 (the max over ~2.6e5 values), MSE 1e-4
 # (RMS error 1e-2), and no worse than 1.5x the error of the reference's own dtype policy (oracle under bf16 autocast).
-# Measured (round 2): max-abs 5.5e-2 .. 6.1e-2, mse 5.5e-5 .. 5.9e-5 (reference bf16 policy: 6.7e-2 / 9.5e-5); thresholds x 1.3.
+# Thresholds = 1.3 x the error of the first implementation of these kernels; the sm_90a kernels are held to the same ones.
 TOL_MAX_ABS = 8e-2
 TOL_MSE = 7.7e-5
 
@@ -93,8 +93,9 @@ def test_small_vae_matches_reference_golden(golden_dir):
     # tiled decode vs the reference's tiled golden
     vae.enable_tiling()
     out_t = vae.decode(z.to("cuda:0"), temporal_chunk=True, window_size=1, tile_sample_min_size=32).sample.float().cpu()
-    assert out_t.shape == g["tiled32"].shape
-    assert (out_t - g["tiled32"]).abs().max().item() < TOL_MAX_ABS
+    tiled32 = torch.load(golden_dir / "vae_small_tiled.pt", weights_only=False)["tiled32"]
+    assert out_t.shape == tiled32.shape
+    assert (out_t - tiled32).abs().max().item() < TOL_MAX_ABS
 
 
 def test_default_width_vae_matches_oracle():

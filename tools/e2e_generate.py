@@ -1,8 +1,8 @@
-"""End-to-end generate() + decode on one or N B200s with synthetic text embeddings and random-init weights:
+"""End-to-end generate() + decode on one or N GPUs with synthetic text embeddings and random-init weights:
 python tools/e2e_generate.py [--height 768 --width 1280 --temp 31]   (BASELINE configs[2]; --temp 16 --height 384 --width 640 = configs[1])
 torchrun --nproc-per-node N tools/e2e_generate.py ...   : every rank runs the same sampler loop (same seeds); the DiT step is
 sharded CFG x sequence-parallel (sp.py) and the VAE decode is context-parallel (temporal split + halo exchange).
-Reports wall-clock frames/s (excluding text encoding, as SURVEY.md §8d defines) and aggregate DiT token-passes/s."""
+Reports wall-clock frames/s (excluding text encoding) and aggregate DiT token-passes/s."""
 import argparse
 import json
 import sys
@@ -72,7 +72,7 @@ lat = sampler.generate(enc, mask, pooled, height=args.height, width=args.width, 
 torch.cuda.synchronize()
 t1 = time.time()
 frames = 1 + 8 * (args.temp - 1)
-res = {"config": f"miniFLUX {args.height}x{args.width}, temp={args.temp} ({frames} frames), steps 20/10, guidance 7/5, {world}xB200 bf16",
+res = {"config": f"miniFLUX {args.height}x{args.width}, temp={args.temp} ({frames} frames), steps 20/10, guidance 7/5, {world} GPU(s), bf16",
        "dit_calls": sampler.dit_calls, "dit_seconds": t1 - t0, "dit_token_passes": tokens[0],
        "dit_token_passes_per_s": tokens[0] / (t1 - t0), "latent_finite": bool(torch.isfinite(lat.float()).all())}
 if vae is not None:

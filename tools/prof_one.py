@@ -22,7 +22,7 @@ if which == "attn":
     sched, pairs = ops.attn_build_schedule(seg, tim)
     ps = ops.attn_build_pair_schedule(sched, S, seg, tim).to(dev)
     sd, td, scd = seg.to(dev), tim.to(dev), sched.to(dev)
-    variant = int(sys.argv[3], 0) if len(sys.argv) > 3 else 0        # pf_attn_desc.variant (0 = default, 3 = one-tile kernel, 0x10 = two-q-tile kernel)
+    variant = int(sys.argv[3], 0) if len(sys.argv) > 3 else 0        # pf_attn_desc.variant (every value runs the same kernel)
     for _ in range(reps):
         ops.attn_fwd(q, k, v, out, sd, td, scd, 0.125, variant=variant, pair_sched=ps)
 elif which == "conv":

@@ -1,5 +1,5 @@
 """torchrun --nproc-per-node N tools/sp_check.py : the CFG x SP parallel DiT step equals the single-GPU step (same kernels,
-same inputs); run on the GPU box with N = 2, 4 or 8."""
+same inputs); run on a node with N = 2, 4 or 8."""
 import os
 import sys
 from pathlib import Path

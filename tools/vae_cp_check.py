@@ -1,5 +1,5 @@
 """torchrun --nproc-per-node N tools/vae_cp_check.py : context-parallel VAE decode (temporal split + per-conv halo
-exchange) equals the single-GPU decode bit for bit, and is timed against it.  Run on the GPU box with N = 2, 4 or 8."""
+exchange) equals the single-GPU decode bit for bit, and is timed against it.  Run on a node with N = 2, 4 or 8."""
 import os
 import sys
 from pathlib import Path
