@@ -35,9 +35,11 @@ PF_API int pf_device_check(void);
 PF_API int pf_warmup(void);
 /* Library options: data-path choices that do not change results (same arithmetic, same bits) but are A/B-measured. */
 enum {
-  PF_OPT_GEMM_STAGED_RESID = 0, /* GATE_RESID epilogue: residual read-modify-write by whole row segments (a warp per row) instead
-                                 * of one thread per row */
-  PF_OPT_GEMM_WAVE_TILING = 1,  /* 64-wide column tiles when their wave count, costed at the measured 0.75 efficiency, beats 128-wide ones */
+  PF_OPT_GEMM_STAGED_RESID = 0, /* GATE_RESID epilogue of the 128-row GEMM kernels: residual read-modify-write by whole row
+                                 * segments (a warp per row) instead of one thread per row.  No effect on the 256 x 128 cluster
+                                 * kernel, whose epilogue works from the accumulator fragments. */
+  PF_OPT_GEMM_WAVE_TILING = 1,  /* with few rows, take the 128 x 128 or 128 x 64 GEMM kernel instead of the 256 x 128 cluster
+                                 * kernel when its wave count x tile area, over its measured relative rate, is smaller */
   /* q-tile grouping hints of pf_attn_fwd_masked.  The sm_90a build has one attention kernel (one q tile per CTA, scores in
    * registers); the three keys are accepted and stored so that existing callers keep working, and change nothing. */
   PF_OPT_ATTN_PAIR_KERNEL = 2,
@@ -143,8 +145,9 @@ typedef struct pf_gemm_desc {
   float norm_eps;
   int32_t heads, head_dim, seq_len;
   int32_t n_split; /* QKV_GELU: first n_split (=3*H*hd) columns are q|k|v */
-  int32_t kernel_variant; /* 0 = auto; 1 = force 128-wide column tiles (n % 128 == 0); 2 = force 64-wide column tiles.
-                           * Same bits either way (same K order); exists so tests can pin each kernel. */
+  int32_t kernel_variant; /* 0 = auto; 1 = force the 256 x 128 two-CTA cluster kernel (n % 128 == 0); 2 = force the 128 x 64
+                           * kernel.  Same bits either way (same K order, same epilogue arithmetic); exists so tests can pin
+                           * each kernel. */
   /* QKV_ROPE under sequence parallelism (peer_count > 1): head h of this rank's token chunk is stored into rank
    * (h / peer_heads)'s buffer peer_qkv[h / peer_heads], laid out [3 (q,k,v)][peer_heads][peer_seq][head_dim], at sequence
    * position peer_row0 + (out_row_begin + m).  q_out/k_out/v_out are ignored.  batches must be 1. */

@@ -141,6 +141,36 @@ __device__ __forceinline__ void tma_load_5d(void* smem_dst, const CUtensorMap* m
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
+// The box lands at the same shared-memory offset in every CTA of `cta_mask`, and each destination CTA's mbarrier at `bar`'s
+// offset receives the complete_tx of its copy.
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                                      uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], "
+      "[%2], %5;" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
+      : "memory");
+}
+
+// ---- thread-block clusters ---------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// arrive on the mbarrier at `bar`'s shared-memory offset in cluster CTA `cta` (this CTA included).  Default (.release.cta)
+// semantics: with .cluster scope the compiler puts a GPU-wide memory barrier in front of every arrive.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t"
+      ".reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
+      "}\n" ::"r"(smem_u32(bar)), "r"(cta)
+      : "memory");
+}
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 
 // ---- warpgroup MMA (wgmma) ---------------------------------------------------
 // One warpgroup (4 warps, 128 threads) issues D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 operands, fp32 accumulators in

@@ -2,11 +2,14 @@
 //
 //   out = epilogue(A[rows, K] . W[N, K]^T + bias)
 //
-// One CTA per SM (persistent, static tile schedule), 384 threads (pf_common.cuh "shared TMA -> wgmma pipeline"):
-//   warpgroup 0 (one lane)  TMA producer: A tile [128 x 64] + W tile [BN x 64] per stage, SWIZZLE_128B, mbarrier tx-count
-//   warpgroups 1, 2         consumers: 4 x wgmma.mma_async (64 x BN x 16) per stage each, fp32 accumulators in registers;
-//                           after the K loop the fragments are staged through shared memory so that the epilogue runs with one
-//                           thread per output row (64 rows x 2 column halves per warpgroup) and stores whole row segments
+// Three kernels, one CTA per SM (persistent, static tile schedule), 384 threads: warpgroup 0 (one lane) is the TMA producer
+// (SWIZZLE_128B boxes, mbarrier tx-count), warpgroups 1 and 2 consume with wgmma.mma_async, fp32 accumulators in registers.
+//   256 x 128 tiles in 2-CTA clusters (every step GEMM; 128 | N): each consumer warpgroup owns 128 rows (2 x m64n128k16 per
+//       k16 step, 128 accumulators per thread); the W box is split between the two producers of a cluster and multicast into
+//       both CTAs; the epilogue runs straight from the accumulator fragments.
+//   128 x 128 and 128 x 64 tiles (pf_common.cuh "shared TMA -> wgmma pipeline"): each consumer warpgroup owns 64 rows; after
+//       the K loop the fragments are staged through shared memory so that the epilogue runs with one thread per output row.
+//       Taken for N not a multiple of 128, and when the wave-quantisation cost model prefers them (few rows).
 // The producer runs ahead into the next tile's stages while the consumers are in the epilogue.
 //
 // Epilogues (include/pf_b200.h PF_EPI_*): bias / GELU-tanh / fp32 store / gate*x+residual / per-head RMSNorm + RoPE
@@ -41,11 +44,18 @@ struct GemmArgs {
   // sequence parallel: q/k/v heads go straight into the owning rank's [3][peer_heads][peer_seq][64] buffer (pf_b200.h)
   __nv_bfloat16* peer_qkv[PF_MAX_PEERS];
   int peer_count, peer_heads, peer_seq, peer_row0;
-  int epi_staged;   // GATE_RESID: whole-row read-modify-write, one warp per row segment (pf_set_option(PF_OPT_GEMM_STAGED_RESID))
+  int epi_staged;   // 128-row kernels' GATE_RESID: whole-row read-modify-write, one warp per row segment (PF_OPT_GEMM_STAGED_RESID)
 };
 
 constexpr int BM = PIPE_BM;
 constexpr int BK = PIPE_BK;
+
+// Relative rates (FLOP/s) of the three kernels, for the wave-quantisation choice in pf_gemm_bf16.  tools/gemm_bench.py on an
+// H100 80GB HBM3 (700 W power limit) at the step's full-size shapes (M = 30720 / 30976): 256 x 128 cluster 456 - 678 TFLOP/s,
+// 1.21 - 1.44 x the 128 x 128 kernel (340 - 489); 128 x 64 0.72 - 0.85 x the 128 x 128 kernel.
+constexpr double GEMM_RATE_CLUSTER = 1.25;
+constexpr double GEMM_RATE_128 = 1.0;
+constexpr double GEMM_RATE_64 = 0.75;
 
 // ---- epilogue helpers (one thread == one output row) -----------------------
 __device__ __forceinline__ void store_bf16x32(__nv_bfloat16* dst, const float (&x)[32]) {
@@ -302,6 +312,282 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_co
   }
 }
 
+// ---- 256 x 128 tiles in 2-CTA clusters ----------------------------------------------------------------------------------
+// The two CTAs of a cluster take adjacent 256-row tiles (same batch, same 128 columns).  Each producer loads its own A box
+// [256 x 64] and half of the W box [64 x 64], multicast into both CTAs, so a stage (32 KB A + 16 KB W) costs each SM 40 KB of
+// L2 -> shared traffic for 4.2 MFLOP.  A stage may be refilled only when the consumers of both CTAs are done with it: every
+// consumer warp arrives on its own and on the peer's empty barrier (16 arrivals per phase).
+constexpr int CBM = 256;
+constexpr int CBN = 128;
+constexpr int C_STAGES = 4;
+constexpr int C_A_BYTES = CBM * BK * 2;
+constexpr int C_B_BYTES = CBN * BK * 2;
+constexpr int C_STAGE_BYTES = C_A_BYTES + C_B_BYTES;
+constexpr int C_SMEM_BYTES = C_STAGES * C_STAGE_BYTES + 1024;
+
+// acc[h][64 x 128] (+)= rows [128 wg + 64 h, +64) of the stage's A box . W box^T, for one tile's K loop
+__device__ __forceinline__ void cluster_consume_tile(float (&acc)[2][64], uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
+                                                     int num_kb, int wg, int& stage, uint32_t& phase) {
+  const int lane = threadIdx.x & 31;
+  int prev = -1;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t sa = smem_u32(smem + stage * C_STAGE_BYTES);
+    const uint64_t da0 = make_smem_desc_kmajor_sw128(sa + (2 * wg + 0) * (64 * 128));
+    const uint64_t da1 = make_smem_desc_kmajor_sw128(sa + (2 * wg + 1) * (64 * 128));
+    const uint64_t db = make_smem_desc_kmajor_sw128(sa + C_A_BYTES);
+    wgmma_reg_fence(acc[0]);
+    wgmma_reg_fence(acc[1]);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BK / 16; ++kk) {
+      const uint32_t accum = (kb | kk) != 0 ? 1u : 0u;
+      wgmma_ss_n128(acc[0], da0 + 2 * kk, db + 2 * kk, accum);
+      wgmma_ss_n128(acc[1], da1 + 2 * kk, db + 2 * kk, accum);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (prev >= 0 && lane == 0) {
+      mbar_arrive_cluster(&empty_bar[prev], 0);
+      mbar_arrive_cluster(&empty_bar[prev], 1);
+    }
+    prev = stage;
+    if (++stage == C_STAGES) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+  wgmma_wait<0>();
+  wgmma_reg_fence(acc[0]);
+  wgmma_reg_fence(acc[1]);
+  if (prev >= 0 && lane == 0) {
+    mbar_arrive_cluster(&empty_bar[prev], 0);
+    mbar_arrive_cluster(&empty_bar[prev], 1);
+  }
+}
+
+// Epilogue straight from the accumulator fragments (pf_common.cuh wgmma layout): thread (warp w, lane l) of consumer
+// warpgroup wg holds, for h, half in {0, 1}, tile row 128 wg + 64 h + 16 w + l / 4 + 8 half at columns 8 i + 2 (l % 4) + {0, 1},
+// i = 0..15, in acc[h][4 i + 2 half + {0, 1}].  Same arithmetic per element, in the same order, as the staged epilogue of the
+// 128-row kernels: the same bits.
+template <int EPI>
+__device__ __forceinline__ void epilogue_frag(const GemmArgs& g, const float (&acc)[2][64], int wg, int b, int m_base, int n_base) {
+  const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const int r_thr = wg * 128 + w * 16 + (lane >> 2);   // + 64 h + 8 half
+  const int c_thr = 2 * (lane & 3);                    // + 8 i
+  bool qkv_tile = (EPI == PF_EPI_QKV_ROPE);
+  if (EPI == PF_EPI_QKV_GELU) qkv_tile = n_base < g.n_split;
+
+  if (qkv_tile) {
+    const int inner = g.heads * g.head_dim;
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {   // the tile's two 64-column heads
+      const int n0 = n_base + hh * 64;
+      const int section = n0 / inner;
+      const int head = (n0 - section * inner) / g.head_dim;
+      __nv_bfloat16* base = section == 0 ? g.q_out : (section == 1 ? g.k_out : g.v_out);
+      const float* nw = section == 0 ? g.q_norm_w : g.k_norm_w;
+#pragma unroll
+      for (int hr = 0; hr < 4; ++hr) {
+        const int h = hr >> 1, half = hr & 1;
+        const int m = m_base + r_thr + 64 * h + 8 * half;
+        const bool valid = m < g.row_count;
+        const int pos = g.out_row_begin + m;
+        float x[16];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          float2 bb = make_float2(0.f, 0.f);
+          if (g.bias != nullptr) bb = __ldg(reinterpret_cast<const float2*>(g.bias + n0 + 8 * j + c_thr));
+          x[2 * j + 0] = acc[h][4 * (8 * hh + j) + 2 * half + 0] + bb.x;
+          x[2 * j + 1] = acc[h][4 * (8 * hh + j) + 2 * half + 1] + bb.y;
+        }
+        if (section < 2) {   // RMSNorm over the head (N:66-79), then RoPE (B:34-39)
+          // The staged epilogue's sum order: chain c (0..3) runs over columns 4 k + c, k ascending, and the head's sum is
+          // (s0 + s1) + (s2 + s3).  Columns 4 k + c alternate between the threads t and t ^ 2 of the row (8 j + 2 t + e
+          // = 4 (2 j + t / 2) + 2 (t % 2) + e), so each thread fetches its partner's values and runs chains 2 (t % 2) + e.
+          const bool lo_first = (lane & 2) == 0;
+          float s_e[2] = {0.f, 0.f};
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float own = x[2 * j + e], other = __shfl_xor_sync(0xffffffffu, own, 2);
+              const float first = lo_first ? own : other, second = lo_first ? other : own;
+              s_e[e] = fmaf(first, first, s_e[e]);
+              s_e[e] = fmaf(second, second, s_e[e]);
+            }
+          }
+          const float pair = s_e[0] + s_e[1];                           // s0 + s1 (t even) or s2 + s3 (t odd)
+          const float ss = pair + __shfl_xor_sync(0xffffffffu, pair, 1);   // fp32 add commutes: same bits in all four
+          const float r = rsqrtf(ss * (1.0f / 64.0f) + g.norm_eps);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const float2 wn = __ldg(reinterpret_cast<const float2*>(nw + 8 * j + c_thr));
+            x[2 * j + 0] *= r * wn.x;
+            x[2 * j + 1] *= r * wn.y;
+          }
+          if (g.rope != nullptr && valid) {
+            const float* rp = g.rope + static_cast<size_t>(pos) * 64 + c_thr;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const float2 cs = __ldg(reinterpret_cast<const float2*>(rp + 8 * j));   // (cos, sin) of pair 4 j + l % 4
+              const float a0 = x[2 * j + 0], a1 = x[2 * j + 1];
+              x[2 * j + 0] = cs.x * a0 - cs.y * a1;
+              x[2 * j + 1] = cs.y * a0 + cs.x * a1;
+            }
+          }
+        }
+        if (valid) {
+          __nv_bfloat16* dst;
+          if (g.peer_count > 1) {
+            const int pr = head / g.peer_heads, hl = head - pr * g.peer_heads;
+            dst = g.peer_qkv[pr] + ((static_cast<size_t>(section) * g.peer_heads + hl) * g.peer_seq + g.peer_row0 + pos) * 64;
+          } else {
+            dst = base + ((static_cast<size_t>(b) * g.heads + head) * g.seq_len + pos) * 64;
+          }
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            *reinterpret_cast<uint32_t*>(dst + 8 * j + c_thr) = pack_bf16x2(x[2 * j + 0], x[2 * j + 1]);
+        }
+      }
+    }
+  } else if (EPI == PF_EPI_GATE_RESID) {
+    // fp32 read-modify-write of the residual: a row's four threads cover 32 contiguous bytes per column group; all 16 loads
+    // of a row are issued before its stores
+    const float* gate = g.gate + b * g.gate_batch_stride + n_base + c_thr;
+    float* obase = reinterpret_cast<float*>(g.out) + g.out_col_begin + n_base + c_thr;
+#pragma unroll
+    for (int hr = 0; hr < 4; ++hr) {
+      const int h = hr >> 1, half = hr & 1;
+      const int m = m_base + r_thr + 64 * h + 8 * half;
+      if (m >= g.row_count) continue;
+      float2* dst = reinterpret_cast<float2*>(obase + (static_cast<size_t>(b) * g.out_batch_rows + g.out_row_begin + m) * g.ldo);
+      float2 rr[16];
+#pragma unroll
+      for (int i = 0; i < 16; ++i) rr[i] = dst[4 * i];
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        float2 bb = make_float2(0.f, 0.f);
+        if (g.bias != nullptr) bb = __ldg(reinterpret_cast<const float2*>(g.bias + n_base + 8 * i + c_thr));
+        const float2 gg = __ldg(reinterpret_cast<const float2*>(gate + 8 * i));
+        const float x0 = acc[h][4 * i + 2 * half + 0] + bb.x;
+        const float x1 = acc[h][4 * i + 2 * half + 1] + bb.y;
+        rr[i].x += gg.x * x0;
+        rr[i].y += gg.y * x1;
+        dst[4 * i] = rr[i];
+      }
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int n = n_base + 8 * i + c_thr;
+      float2 bb = make_float2(0.f, 0.f);
+      if (g.bias != nullptr) bb = __ldg(reinterpret_cast<const float2*>(g.bias + n));
+#pragma unroll
+      for (int hr = 0; hr < 4; ++hr) {
+        const int h = hr >> 1, half = hr & 1;
+        const int m = m_base + r_thr + 64 * h + 8 * half;
+        float x0 = acc[h][4 * i + 2 * half + 0] + bb.x;
+        float x1 = acc[h][4 * i + 2 * half + 1] + bb.y;
+        if (EPI == PF_EPI_GELU_BF16 || EPI == PF_EPI_QKV_GELU) {
+          x0 = gelu_tanh_f(x0);
+          x1 = gelu_tanh_f(x1);
+        }
+        if (m >= g.row_count) continue;
+        const size_t out_row = static_cast<size_t>(b) * g.out_batch_rows + g.out_row_begin + m;
+        if (EPI == PF_EPI_STORE_F32) {
+          *reinterpret_cast<float2*>(reinterpret_cast<float*>(g.out) + out_row * g.ldo + g.out_col_begin + n) = make_float2(x0, x1);
+        } else {
+          const int col = (EPI == PF_EPI_QKV_GELU) ? (g.out_col_begin + n - g.n_split) : (g.out_col_begin + n);
+          *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(g.out) + out_row * g.ldo + col) = pack_bf16x2(x0, x1);
+        }
+      }
+    }
+  }
+}
+
+template <int EPI>
+__global__ void __launch_bounds__(PIPE_THREADS, 1)
+gemm_bf16_cluster_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
+                         const GemmArgs g) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+
+  __shared__ __align__(8) uint64_t full_bar[C_STAGES];
+  __shared__ __align__(8) uint64_t empty_bar[C_STAGES];
+
+  const int warp = threadIdx.x >> 5;
+  const int wgroup = warp >> 2;
+  const uint32_t rank = cluster_ctarank();
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tm_a);
+    tma_prefetch_desc(&tm_b);
+    for (int i = 0; i < C_STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2 * PIPE_CONSUMER_WARPS);
+    }
+    fence_barrier_init();
+  }
+  // the peer's barriers are initialised before anything arrives on them or multicasts into its shared memory
+  cluster_arrive();
+  cluster_wait();
+
+  // Static schedule over tile pairs: both CTAs of a cluster walk the same pairs.  m_tiles is even-padded per batch; the
+  // partner of an odd last tile loads rows past row_count (zero-filled or masked) and stores nothing.
+  const int num_kb = (g.k + BK - 1) / BK;
+  const int m_pairs = (g.m_tiles + 1) >> 1;
+  const int pairs_per_batch = m_pairs * g.n_tiles;
+  const int total_pairs = g.batches * pairs_per_batch;
+  const int cluster = blockIdx.x >> 1, clusters = gridDim.x >> 1;
+
+  if (wgroup == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
+      // ===== TMA producer =====
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int p = cluster; p < total_pairs; p += clusters) {
+        const int b = p / pairs_per_batch;
+        const int r = p - b * pairs_per_batch;
+        const int mt = 2 * (r / g.n_tiles) + static_cast<int>(rank);
+        const int nt = r % g.n_tiles;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * C_STAGE_BYTES;
+          mbar_arrive_expect_tx(&full_bar[stage], C_STAGE_BYTES);
+          tma_load_3d(sa, &tm_a, &full_bar[stage], kb * BK, g.row_begin + mt * CBM, b);
+          tma_load_2d_multicast(sa + C_A_BYTES + rank * (C_B_BYTES / 2), &tm_b, &full_bar[stage], kb * BK,
+                                nt * CBN + rank * (CBN / 2), 0x3);
+          if (++stage == C_STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    }
+    __syncwarp();
+  } else {
+    // ===== consumers: each warpgroup owns 128 rows of the tile =====
+    setmaxnreg_inc<232>();
+    const int wg = wgroup - 1;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[2][64];
+    for (int p = cluster; p < total_pairs; p += clusters) {
+      const int b = p / pairs_per_batch;
+      const int r = p - b * pairs_per_batch;
+      const int mt = 2 * (r / g.n_tiles) + static_cast<int>(rank);
+      const int nt = r % g.n_tiles;
+      cluster_consume_tile(acc, smem, full_bar, empty_bar, num_kb, wg, stage, phase);
+      epilogue_frag<EPI>(g, acc, wg, b, mt * CBM, nt * CBN);
+    }
+  }
+  // no CTA exits while its peer may still arrive on its barriers
+  cluster_arrive();
+  cluster_wait();
+}
+
 template <int BN, int EPI>
 static int launch_gemm(const CUtensorMap& tm_a, const CUtensorMap& tm_b, const GemmArgs& g, cudaStream_t stream) {
   using Cfg = PipeCfg<BN>;
@@ -315,19 +601,73 @@ static int launch_gemm(const CUtensorMap& tm_a, const CUtensorMap& tm_b, const G
   return check_launch("pf_gemm_bf16");
 }
 
+// Clusters of the 256 x 128 kernel that fit on the device at once (SMs pair up within a GPC, so this can be below
+// num_sms() / 2); queried once, before any CUDA-graph capture, by warmup_gemm.
+static int g_cluster_slots = 0;
+
+static int cluster_slots() {
+  if (g_cluster_slots > 0) return g_cluster_slots;
+  auto kern = gemm_bf16_cluster_kernel<PF_EPI_STORE_BF16>;
+  if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), C_SMEM_BYTES, "gemm cluster")) return rc;
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.gridDim = dim3(2, 1, 1);
+  cfg.blockDim = dim3(PIPE_THREADS, 1, 1);
+  cfg.dynamicSmemBytes = C_SMEM_BYTES;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  int n = 0;
+  if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n <= 0) {
+    (void)cudaGetLastError();
+    n = num_sms() > 0 ? num_sms() / 2 : 66;
+  }
+  g_cluster_slots = n;
+  return n;
+}
+
 template <int EPI>
-static int dispatch_bn(int bn, const CUtensorMap& tm_a, const CUtensorMap& tm_b, const GemmArgs& g, cudaStream_t stream) {
-  switch (bn) {
+static int launch_cluster(const CUtensorMap& tm_a, const CUtensorMap& tm_b, const GemmArgs& g, cudaStream_t stream) {
+  auto kern = gemm_bf16_cluster_kernel<EPI>;
+  if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), C_SMEM_BYTES, "gemm cluster")) return rc;
+  const int slots = cluster_slots();
+  if (slots < 0) return slots;
+  const int pairs = g.batches * ((g.m_tiles + 1) / 2) * g.n_tiles;
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.gridDim = dim3(2 * (pairs < slots ? pairs : slots), 1, 1);
+  cfg.blockDim = dim3(PIPE_THREADS, 1, 1);
+  cfg.dynamicSmemBytes = C_SMEM_BYTES;
+  cfg.stream = stream;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  (void)cudaLaunchKernelEx(&cfg, kern, tm_a, tm_b, g);
+  return check_launch("pf_gemm_bf16");
+}
+
+// tile 0 = 256 x 128 in 2-CTA clusters, else the 128-row kernel with BLOCK_N = tile
+template <int EPI>
+static int dispatch_tile(int tile, const CUtensorMap& tm_a, const CUtensorMap& tm_b, const GemmArgs& g, cudaStream_t stream) {
+  switch (tile) {
+    case 0: return launch_cluster<EPI>(tm_a, tm_b, g, stream);
     case 128: return launch_gemm<128, EPI>(tm_a, tm_b, g, stream);
     case 64: return launch_gemm<64, EPI>(tm_a, tm_b, g, stream);
   }
-  set_error("unsupported BLOCK_N %d", bn);
+  set_error("unsupported GEMM tile %d", tile);
   return -1;
 }
 
 template <int EPI>
 static int warm_epi() {
-  int rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_bf16_wgmma_kernel<128, EPI>), PipeCfg<128>::SMEM_BYTES, "gemm<128>");
+  int rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_bf16_cluster_kernel<EPI>), C_SMEM_BYTES, "gemm cluster");
+  if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_bf16_wgmma_kernel<128, EPI>), PipeCfg<128>::SMEM_BYTES, "gemm<128>");
   if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_bf16_wgmma_kernel<64, EPI>), PipeCfg<64>::SMEM_BYTES, "gemm<64>");
   return rc;
 }
@@ -340,6 +680,7 @@ int warmup_gemm() {
   if (!rc) rc = warm_epi<PF_EPI_GATE_RESID>();
   if (!rc) rc = warm_epi<PF_EPI_QKV_ROPE>();
   if (!rc) rc = warm_epi<PF_EPI_QKV_GELU>();
+  if (!rc) rc = cluster_slots() > 0 ? 0 : -1;
   return rc;
 }
 
@@ -361,8 +702,8 @@ extern "C" int pf_gemm_bf16(const pf_gemm_desc* d, void* stream_) {
   const int epi = d->epilogue;
   PF_REQUIRE(epi >= 0 && epi <= PF_EPI_QKV_GELU, "pf_gemm_bf16: unknown epilogue %d", epi);
 
-  // Column tiling: 128-wide tiles (64 x 128 fp32 accumulators per consumer warpgroup) when they divide n, else 64-wide.  The QKV
-  // epilogues work per 64-column head, so any multiple of 64 is head-aligned.
+  // Column tiling: 128-wide tiles when they divide n, else 64-wide.  The QKV epilogues work per 64-column head, so any
+  // multiple of 64 is head-aligned.
   int bn = 0;
   const bool qkv = (epi == PF_EPI_QKV_ROPE || epi == PF_EPI_QKV_GELU);
   if (qkv) {
@@ -395,7 +736,6 @@ extern "C" int pf_gemm_bf16(const pf_gemm_desc* d, void* stream_) {
   g.row_count = d->row_count;
   g.n = d->n;
   g.k = d->k;
-  g.m_tiles = (d->row_count + BM - 1) / BM;
   g.bias = d->bias;
   g.out = d->out;
   g.ldo = d->ldo;
@@ -429,32 +769,38 @@ extern "C" int pf_gemm_bf16(const pf_gemm_desc* d, void* stream_) {
     for (int i = 0; i < d->peer_count; ++i) PF_REQUIRE(d->peer_qkv[i] != nullptr, "pf_gemm_bf16: peer_qkv[%d] is null", i);
   }
 
-  // kernel_variant 1 / 2 pins the 128-wide / 64-wide tile kernel
+  // Kernels: tile 0 = 256 x 128 in 2-CTA clusters (needs 128 | n), 128 = 128 x 128, 64 = 128 x 64.  All three run the same
+  // wgmma k16 steps in the same order per output element and the same epilogue arithmetic: same bits whichever runs.
+  // kernel_variant 1 pins the 256 x 128 cluster kernel, 2 the 128 x 64 kernel.
   PF_REQUIRE(d->kernel_variant >= 0 && d->kernel_variant <= 2, "pf_gemm_bf16: bad kernel_variant %d", d->kernel_variant);
   PF_REQUIRE(d->kernel_variant != 1 || bn == 128, "pf_gemm_bf16: kernel_variant 1 (128-wide tiles) needs n %% 128 == 0");
-  if (d->kernel_variant == 2) bn = 64;
-  // Wave quantisation: with few rows (a sequence-parallel rank's chunk) the last wave of the persistent grid can be mostly
-  // idle.  The 64-wide tiling changes neither the K order nor the bits, so take it when its waves x tile width, over the
-  // 64-wide kernel's efficiency, is smaller.  Efficiency 0.75 of the 128-wide kernel: measured on an H100 80GB HBM3 (700 W) at
-  // M = 30976, K = 1920 / 7680, N = 1920 / 7680, where the same GEMMs took 1.33 - 1.37 x as long with 64-wide tiles
-  // (bench.py per-family breakdown, e.g. ff2 15.2 -> 20.5 ms, single_out 34.2 -> 46.9 ms).
-  if (bn == 128 && d->kernel_variant == 0 && get_option(PF_OPT_GEMM_WAVE_TILING)) {
+  int tile = bn == 128 ? 0 : 64;
+  if (d->kernel_variant == 2) tile = 64;
+  // Wave quantisation: with few rows (the 128-row text ranges, a sequence-parallel rank's chunk) the big tiles leave most of
+  // the last (or only) wave of the persistent grid idle.  Take the kernel with the least waves x tile area / relative rate.
+  if (tile == 0 && d->kernel_variant == 0 && get_option(PF_OPT_GEMM_WAVE_TILING)) {
     int sms = num_sms();
     if (sms <= 0) sms = 132;
-    auto cost = [&](int tile_n) -> double {
-      const long long tiles = static_cast<long long>(d->batches) * ((d->row_count + BM - 1) / BM) * (d->n / tile_n);
-      const long long waves = (tiles + sms - 1) / sms;
-      return static_cast<double>(waves) * tile_n / (tile_n == 128 ? 1.0 : 0.75);
-    };
-    if (cost(64) < cost(128)) bn = 64;
+    const int slots = cluster_slots();
+    const long long mt128 = (d->row_count + BM - 1) / BM, mt256 = (d->row_count + CBM - 1) / CBM;
+    const long long waves0 = (d->batches * ((mt256 + 1) / 2) * (d->n / 128) + slots - 1) / (slots > 0 ? slots : 66);
+    const long long waves128 = (d->batches * mt128 * (d->n / 128) + sms - 1) / sms;
+    const long long waves64 = (d->batches * mt128 * (d->n / 64) + sms - 1) / sms;
+    const double cost0 = waves0 * 2.0 / GEMM_RATE_CLUSTER, cost128 = waves128 * 1.0 / GEMM_RATE_128,
+                 cost64 = waves64 * 0.5 / GEMM_RATE_64;
+    if (cost128 < cost0 && cost128 <= cost64) tile = 128;
+    else if (cost64 < cost0) tile = 64;
   }
+  if (tile != 0) bn = tile;
+  const int tile_rows = tile == 0 ? CBM : BM;
+  g.m_tiles = (d->row_count + tile_rows - 1) / tile_rows;
   CUtensorMap tm_a;
   {
     const uint64_t dims[3] = {static_cast<uint64_t>(d->k), static_cast<uint64_t>(d->rows_per_batch),
                               static_cast<uint64_t>(d->batches)};
     const uint64_t strides[2] = {static_cast<uint64_t>(d->lda) * 2,
                                  static_cast<uint64_t>(d->lda) * 2 * static_cast<uint64_t>(d->rows_per_batch)};
-    const uint32_t box[3] = {BK, BM, 1};
+    const uint32_t box[3] = {BK, static_cast<uint32_t>(tile_rows), 1};
     int rc = encode_tensor_map(&tm_a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, d->a, dims, strides, box,
                                CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
@@ -464,19 +810,19 @@ extern "C" int pf_gemm_bf16(const pf_gemm_desc* d, void* stream_) {
   {
     const uint64_t dims[2] = {static_cast<uint64_t>(d->k), static_cast<uint64_t>(d->n)};
     const uint64_t strides[1] = {static_cast<uint64_t>(d->k) * 2};
-    const uint32_t box[2] = {BK, static_cast<uint32_t>(bn)};
+    const uint32_t box[2] = {BK, static_cast<uint32_t>(tile == 0 ? CBN / 2 : bn)};   // cluster: each CTA loads half
     int rc = encode_tensor_map(&tm_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, d->w, dims, strides, box,
                                CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
   g.n_tiles = d->n / bn;
   switch (epi) {
-    case PF_EPI_STORE_BF16: return dispatch_bn<PF_EPI_STORE_BF16>(bn, tm_a, tm_b, g, stream);
-    case PF_EPI_GELU_BF16: return dispatch_bn<PF_EPI_GELU_BF16>(bn, tm_a, tm_b, g, stream);
-    case PF_EPI_STORE_F32: return dispatch_bn<PF_EPI_STORE_F32>(bn, tm_a, tm_b, g, stream);
-    case PF_EPI_GATE_RESID: return dispatch_bn<PF_EPI_GATE_RESID>(bn, tm_a, tm_b, g, stream);
-    case PF_EPI_QKV_ROPE: return dispatch_bn<PF_EPI_QKV_ROPE>(bn, tm_a, tm_b, g, stream);
-    case PF_EPI_QKV_GELU: return dispatch_bn<PF_EPI_QKV_GELU>(bn, tm_a, tm_b, g, stream);
+    case PF_EPI_STORE_BF16: return dispatch_tile<PF_EPI_STORE_BF16>(tile, tm_a, tm_b, g, stream);
+    case PF_EPI_GELU_BF16: return dispatch_tile<PF_EPI_GELU_BF16>(tile, tm_a, tm_b, g, stream);
+    case PF_EPI_STORE_F32: return dispatch_tile<PF_EPI_STORE_F32>(tile, tm_a, tm_b, g, stream);
+    case PF_EPI_GATE_RESID: return dispatch_tile<PF_EPI_GATE_RESID>(tile, tm_a, tm_b, g, stream);
+    case PF_EPI_QKV_ROPE: return dispatch_tile<PF_EPI_QKV_ROPE>(tile, tm_a, tm_b, g, stream);
+    case PF_EPI_QKV_GELU: return dispatch_tile<PF_EPI_QKV_GELU>(tile, tm_a, tm_b, g, stream);
   }
   return -1;
 }
