@@ -157,6 +157,32 @@ typedef struct pf_gemm_desc {
 
 PF_API int pf_gemm_bf16(const pf_gemm_desc* desc, void* stream);
 
+/* ------------------------------------------------------------------ FP8 (e4m3) GEMM and its quantisers (opt-in)
+ * Numerical contract.  e4m3 = float8_e4m3fn: max finite 448, round to nearest even, saturating (F2FP.SATFINITE.E4M3).
+ *   Quantising a row x[0..K) (activations: one scale per token; weights: one scale per output channel, the same formula):
+ *     amax = max_k |x[k]|;  inv = amax > 0 ? 448.f / amax : 0.f (IEEE fp32 division);  q[k] = e4m3(x[k] * inv);
+ *     scale = amax / 448.f.  A row of zeros gives zeros and scale 0; no NaN or Inf.  |x[k] * inv| <= 448 (1 + 2^-23), which
+ *     rounds to 448, so a host restatement that casts with torch (which does not saturate) gives the same bits.
+ *   GEMM:  acc[r, n] = sum_k q_a[r, k] q_w[n, k] in fp32, then y = acc * scale_a[r] * scale_w[n] + bias[n], and y goes into
+ *     the epilogue exactly as in pf_gemm_bf16 (every PF_EPI_*).  Hopper's fp8 wgmma adds into its accumulator with reduced
+ *     internal precision, so the kernel adds the partial sum of every K = 128 slice into the fp32 accumulator separately
+ *     (promotion); the sum order depends on K only (a row's outputs do not depend on the launch's row range).
+ *
+ * pf_gemm_fp8: the pf_gemm_bf16 descriptor with d->a, d->w pointing to e4m3 data (lda counts elements = bytes);
+ * a_row_scale fp32 [batches, rows_per_batch] indexed like A's rows, w_col_scale fp32 [n].  Requires n % 128 == 0,
+ * k % 16 == 0, lda % 16 == 0, kernel_variant 0 and no peer stores (peer_count 0). */
+PF_API int pf_gemm_fp8(const pf_gemm_desc* desc, const float* a_row_scale, const float* w_col_scale, void* stream);
+/* pf_ln_modulate with an e4m3 output: the fp32 LN-modulated row is quantised directly (one rounding) with the contract above;
+ * y_fp8 row stride = dim; row_scale fp32 [batches, rows_per_batch] (rows outside the range are not written). */
+PF_API int pf_ln_modulate_fp8(const float* x, void* y_fp8, float* row_scale, int32_t batches, int32_t rows_per_batch,
+                              int32_t row_begin, int32_t row_count, int32_t dim, const float* shift, const float* scale,
+                              int64_t mod_batch_stride, float eps, void* stream);
+/* Row quantiser: bf16 x[r, 0..cols) (row stride ldx) -> e4m3 y[r, ...] (row stride ldy) + row_scale[r], for the rows
+ * r = b * rows_per_batch + row_begin + m, m < row_count.  cols % 8 == 0, ldx % 8 == 0, ldy % 8 == 0, 16-byte aligned x and
+ * 8-byte aligned y. */
+PF_API int pf_quantize_rows_fp8(const void* x_bf16, int64_t ldx, void* y_fp8, int64_t ldy, float* row_scale, int32_t batches,
+                                int32_t rows_per_batch, int32_t row_begin, int32_t row_count, int32_t cols, void* stream);
+
 /* ------------------------------------------------------------------ masked joint attention (wgmma + TMA)
  * softmax(Q K^T * scale + mask) V with mask(q, kv) = (seg[q] == seg[kv]) && (time[q] >= time[kv])  (F:318-350),
  * replacing F.scaled_dot_product_attention with the dense bool mask at B:363-365 and B:596-598.

@@ -15,7 +15,7 @@ LIB_PATH = _HERE / "lib" / "libpf_b200.so"
 # every symbol include/pf_b200.h declares (tests check the .so exports exactly these)
 SYMBOLS = [
     "pf_last_error", "pf_version", "pf_device_check", "pf_warmup", "pf_set_option", "pf_get_option", "pf_launch_count",
-    "pf_gemm_bf16",
+    "pf_gemm_bf16", "pf_gemm_fp8", "pf_ln_modulate_fp8", "pf_quantize_rows_fp8",
     "pf_attn_build_schedule", "pf_attn_build_pair_schedule", "pf_attn_build_pair_masks", "pf_attn_build_group_schedule",
     "pf_attn_build_group_masks", "pf_attn_fwd_masked",
     "pf_ln_modulate", "pf_small_linear", "pf_timestep_embedding",
@@ -103,6 +103,11 @@ def load() -> C.CDLL:
     lib.pf_last_error.restype = C.c_char_p
     lib.pf_launch_count.restype = C.c_int64
     lib.pf_gemm_bf16.argtypes = [C.POINTER(GemmDesc), C.c_void_p]
+    lib.pf_gemm_fp8.argtypes = [C.POINTER(GemmDesc), C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.pf_ln_modulate_fp8.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                       C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_void_p]
+    lib.pf_quantize_rows_fp8.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int32,
+                                         C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     lib.pf_attn_fwd_masked.argtypes = [C.POINTER(AttnDesc), C.c_void_p]
     lib.pf_attn_build_schedule.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     lib.pf_attn_build_pair_schedule.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]

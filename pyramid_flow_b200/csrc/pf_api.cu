@@ -246,7 +246,7 @@ int pf_warmup(void) {
 }
 
 const char* pf_last_error(void) { return pf::g_err; }
-int pf_version(void) { return 200; }
+int pf_version(void) { return 201; }
 int64_t pf_launch_count(void) { return pf::g_launches.load(); }
 
 int pf_device_check(void) {

@@ -1,6 +1,8 @@
 // pf_elementwise.cu — the HBM-bound kernels of the DiT step: LayerNorm+AdaLN modulate pre-pass, the small-M linear
 // (all-layer AdaLN modulation GEMV + conditioning MLPs), timestep sinusoid, patchify / unpatchify, CFG+Euler.
 // Reference op sites are cited in include/pf_b200.h next to each entry point.
+#include <cuda_fp8.h>
+
 #include "../../include/pf_b200.h"
 #include "pf_common.cuh"
 
@@ -8,13 +10,28 @@ namespace pf {
 
 // ---------------------------------------------------------------------------------------------------------------
 // LN + modulate: one warp per row, row kept in registers (dim <= 2048, dim % 128 == 0), 128-bit loads, 64-bit stores.
-// Algorithmic traffic: 4 B (fp32 in) + 2 B (bf16 out) per element.
+// Algorithmic traffic: 4 B (fp32 in) + 2 B (bf16 out) per element; with the e4m3 output (FP8) 4 B + 1 B, and the row's amax
+// is one more warp reduction over the values already in registers (pf_b200.h FP8 contract).
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int LN_MAX_VEC = 16;  // float4 per lane
+constexpr float E4M3_MAX = 448.f;
 
+// e4m3 bytes of (a, b, c, d) * inv, packed little-endian (pf_b200.h FP8 contract)
+__device__ __forceinline__ uint32_t e4m3x4(float a, float b, float c, float d, float inv) {
+  const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(a * inv, b * inv), __NV_SATFINITE, __NV_E4M3);
+  const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(c * inv, d * inv), __NV_SATFINITE, __NV_E4M3);
+  return lo | (hi << 16);
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+template <bool FP8>
 __global__ void __launch_bounds__(256)
-ln_modulate_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, int batches, int rows_per_batch,
-                   int row_begin, int row_count, int dim, const float* __restrict__ shift,
+ln_modulate_kernel(const float* __restrict__ x, void* __restrict__ y_, float* __restrict__ row_scale, int batches,
+                   int rows_per_batch, int row_begin, int row_count, int dim, const float* __restrict__ shift,
                    const float* __restrict__ scale, long long mod_batch_stride, float eps) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
@@ -52,19 +69,81 @@ ln_modulate_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, i
 
   const float4* sh4 = reinterpret_cast<const float4*>(shift + b * mod_batch_stride);
   const float4* sc4 = reinterpret_cast<const float4*>(scale + b * mod_batch_stride);
-  uint2* y2 = reinterpret_cast<uint2*>(y + row * dim);
+  if constexpr (!FP8) {
+    uint2* y2 = reinterpret_cast<uint2*>(static_cast<__nv_bfloat16*>(y_) + row * dim);
 #pragma unroll
-  for (int i = 0; i < LN_MAX_VEC; ++i) {
-    if (i < nvec) {
-      const float4 sh = __ldg(sh4 + i * 32 + lane);
-      const float4 sc = __ldg(sc4 + i * 32 + lane);
-      const float o0 = (v[i].x - mean) * rstd * (1.f + sc.x) + sh.x;
-      const float o1 = (v[i].y - mean) * rstd * (1.f + sc.y) + sh.y;
-      const float o2 = (v[i].z - mean) * rstd * (1.f + sc.z) + sh.z;
-      const float o3 = (v[i].w - mean) * rstd * (1.f + sc.w) + sh.w;
-      y2[i * 32 + lane] = make_uint2(pack_bf16x2(o0, o1), pack_bf16x2(o2, o3));
+    for (int i = 0; i < LN_MAX_VEC; ++i) {
+      if (i < nvec) {
+        const float4 sh = __ldg(sh4 + i * 32 + lane);
+        const float4 sc = __ldg(sc4 + i * 32 + lane);
+        const float o0 = (v[i].x - mean) * rstd * (1.f + sc.x) + sh.x;
+        const float o1 = (v[i].y - mean) * rstd * (1.f + sc.y) + sh.y;
+        const float o2 = (v[i].z - mean) * rstd * (1.f + sc.z) + sh.z;
+        const float o3 = (v[i].w - mean) * rstd * (1.f + sc.w) + sh.w;
+        y2[i * 32 + lane] = make_uint2(pack_bf16x2(o0, o1), pack_bf16x2(o2, o3));
+      }
     }
+  } else {
+    float amax = 0.f;
+#pragma unroll
+    for (int i = 0; i < LN_MAX_VEC; ++i) {
+      if (i < nvec) {
+        const float4 sh = __ldg(sh4 + i * 32 + lane);
+        const float4 sc = __ldg(sc4 + i * 32 + lane);
+        v[i].x = (v[i].x - mean) * rstd * (1.f + sc.x) + sh.x;
+        v[i].y = (v[i].y - mean) * rstd * (1.f + sc.y) + sh.y;
+        v[i].z = (v[i].z - mean) * rstd * (1.f + sc.z) + sh.z;
+        v[i].w = (v[i].w - mean) * rstd * (1.f + sc.w) + sh.w;
+        amax = fmaxf(amax, fmaxf(fmaxf(fabsf(v[i].x), fabsf(v[i].y)), fmaxf(fabsf(v[i].z), fabsf(v[i].w))));
+      }
+    }
+    amax = warp_max(amax);
+    const float inv = amax > 0.f ? E4M3_MAX / amax : 0.f;
+    uint32_t* y4 = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(y_) + row * dim);
+#pragma unroll
+    for (int i = 0; i < LN_MAX_VEC; ++i)
+      if (i < nvec) y4[i * 32 + lane] = e4m3x4(v[i].x, v[i].y, v[i].z, v[i].w, inv);
+    if (lane == 0) row_scale[row] = amax / E4M3_MAX;
   }
+}
+
+// Row quantiser bf16 -> e4m3 + row scale (pf_b200.h FP8 contract): one warp per row, two passes over the row (amax, then
+// quantise; the second read is served by L1 / L2), 16-byte loads and 8-byte stores.  cols % 8 == 0.
+__global__ void __launch_bounds__(256)
+quantize_rows_fp8_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, uint8_t* __restrict__ y, long long ldy,
+                         float* __restrict__ row_scale, int rows_per_batch, int row_begin, int row_count, int total, int cols) {
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (warp >= total) return;
+  const int b = warp / row_count;
+  const size_t row = static_cast<size_t>(b) * rows_per_batch + row_begin + (warp - b * row_count);
+  const uint4* x8 = reinterpret_cast<const uint4*>(x + row * ldx);
+  uint2* y8 = reinterpret_cast<uint2*>(y + row * ldy);
+  const int nchunk = cols >> 3;
+  auto unpack = [](const uint4& u, float (&f)[8]) {
+    const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float2 p = __bfloat1622float2(h[i]);
+      f[2 * i] = p.x;
+      f[2 * i + 1] = p.y;
+    }
+  };
+  float amax = 0.f;
+  for (int c = lane; c < nchunk; c += 32) {
+    float f[8];
+    unpack(x8[c], f);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) amax = fmaxf(amax, fabsf(f[i]));
+  }
+  amax = warp_max(amax);
+  const float inv = amax > 0.f ? E4M3_MAX / amax : 0.f;
+  for (int c = lane; c < nchunk; c += 32) {
+    float f[8];
+    unpack(x8[c], f);
+    y8[c] = make_uint2(e4m3x4(f[0], f[1], f[2], f[3], inv), e4m3x4(f[4], f[5], f[6], f[7], inv));
+  }
+  if (lane == 0) row_scale[row] = amax / E4M3_MAX;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -267,10 +346,45 @@ int pf_ln_modulate(const float* x, void* y, int32_t batches, int32_t rows_per_ba
   PF_REQUIRE(mod_batch_stride % 4 == 0, "pf_ln_modulate: modulation stride must be a multiple of 4 floats");
   const long long warps = static_cast<long long>(batches) * row_count;
   const int blocks = static_cast<int>((warps + 7) / 8);
-  ln_modulate_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      x, static_cast<__nv_bfloat16*>(y), batches, rows_per_batch, row_begin, row_count, dim, shift, scale,
-      mod_batch_stride, eps);
+  ln_modulate_kernel<false><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      x, y, nullptr, batches, rows_per_batch, row_begin, row_count, dim, shift, scale, mod_batch_stride, eps);
   return check_launch("pf_ln_modulate");
+}
+
+int pf_ln_modulate_fp8(const float* x, void* y, float* row_scale, int32_t batches, int32_t rows_per_batch, int32_t row_begin,
+                       int32_t row_count, int32_t dim, const float* shift, const float* scale, int64_t mod_batch_stride,
+                       float eps, void* stream) {
+  using namespace pf;
+  PF_REQUIRE(x && y && row_scale && shift && scale, "pf_ln_modulate_fp8: null pointer");
+  PF_REQUIRE(dim % 128 == 0 && dim <= 128 * LN_MAX_VEC, "pf_ln_modulate_fp8: dim=%d must be a multiple of 128 and <= %d", dim, 128 * LN_MAX_VEC);
+  PF_REQUIRE(batches > 0 && row_count > 0 && row_begin >= 0 && row_begin + row_count <= rows_per_batch, "pf_ln_modulate_fp8: bad row range");
+  PF_REQUIRE(mod_batch_stride % 4 == 0, "pf_ln_modulate_fp8: modulation stride must be a multiple of 4 floats");
+  const long long warps = static_cast<long long>(batches) * row_count;
+  const int blocks = static_cast<int>((warps + 7) / 8);
+  ln_modulate_kernel<true><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      x, y, row_scale, batches, rows_per_batch, row_begin, row_count, dim, shift, scale, mod_batch_stride, eps);
+  return check_launch("pf_ln_modulate_fp8");
+}
+
+int pf_quantize_rows_fp8(const void* x, int64_t ldx, void* y, int64_t ldy, float* row_scale, int32_t batches,
+                         int32_t rows_per_batch, int32_t row_begin, int32_t row_count, int32_t cols, void* stream) {
+  using namespace pf;
+  PF_REQUIRE(x && y && row_scale, "pf_quantize_rows_fp8: null pointer");
+  PF_REQUIRE(cols > 0 && cols % 8 == 0, "pf_quantize_rows_fp8: cols=%d must be a positive multiple of 8", cols);
+  PF_REQUIRE(ldx % 8 == 0 && ldx >= cols && ldy % 8 == 0 && ldy >= cols,
+             "pf_quantize_rows_fp8: ldx=%lld and ldy=%lld must be >= cols and multiples of 8", (long long)ldx, (long long)ldy);
+  PF_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 7) == 0,
+             "pf_quantize_rows_fp8: x must be 16-byte and y 8-byte aligned");
+  PF_REQUIRE(batches > 0 && row_count > 0 && row_begin >= 0 && row_begin + row_count <= rows_per_batch,
+             "pf_quantize_rows_fp8: bad row range (batches %d rows %d begin %d count %d)", batches, rows_per_batch, row_begin,
+             row_count);
+  const long long warps = static_cast<long long>(batches) * row_count;
+  PF_REQUIRE(warps < (1LL << 31) - 255, "pf_quantize_rows_fp8: too many rows");
+  const int blocks = static_cast<int>((warps + 7) / 8);
+  quantize_rows_fp8_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const __nv_bfloat16*>(x), ldx, static_cast<uint8_t*>(y), ldy, row_scale, rows_per_batch, row_begin,
+      row_count, static_cast<int>(warps), cols);
+  return check_launch("pf_quantize_rows_fp8");
 }
 
 int pf_small_linear(const float* x, int32_t m, int32_t k, const void* w, const float* bias, int32_t n, float* y,

@@ -14,6 +14,9 @@
 //
 // Epilogues (include/pf_b200.h PF_EPI_*): bias / GELU-tanh / fp32 store / gate*x+residual / per-head RMSNorm + RoPE
 // with head-major Q,K,V stores / the single-block fused q|k|v|mlp split.
+// pf_gemm_fp8 runs the cluster kernel on e4m3 operands: 128 x 128 tiles (one 64-row half per consumer warpgroup), K = 128
+// per stage, per-stage promotion of the fp8 partial sums into fp32, and the same epilogues after the per-row x per-column
+// dequantisation scale.
 // Reference op sites are listed in include/pf_b200.h at pf_gemm_bf16.
 #include <cstdlib>
 
@@ -45,6 +48,10 @@ struct GemmArgs {
   __nv_bfloat16* peer_qkv[PF_MAX_PEERS];
   int peer_count, peer_heads, peer_seq, peer_row0;
   int epi_staged;   // 128-row kernels' GATE_RESID: whole-row read-modify-write, one warp per row segment (PF_OPT_GEMM_STAGED_RESID)
+  // e4m3 operands (pf_gemm_fp8): a_scale[b * rows_per_batch + row_begin + m], w_scale[n]
+  const float* a_scale;
+  const float* w_scale;
+  int rows_per_batch;
 };
 
 constexpr int BM = PIPE_BM;
@@ -319,23 +326,37 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_co
 // consumer warp arrives on its own and on the peer's empty barrier (16 arrivals per phase).
 constexpr int CBM = 256;
 constexpr int CBN = 128;
-constexpr int C_STAGES = 4;
-constexpr int C_A_BYTES = CBM * BK * 2;
-constexpr int C_B_BYTES = CBN * BK * 2;
-constexpr int C_STAGE_BYTES = C_A_BYTES + C_B_BYTES;
-constexpr int C_SMEM_BYTES = C_STAGES * C_STAGE_BYTES + 1024;
+// The cluster kernel's two operand types.  A stage row is one 128-byte swizzle row of K in both: 64 bf16 or 128 e4m3.
+//   bf16: 256-row tiles; each consumer warpgroup owns two 64-row halves (H = 2).
+//   e4m3: 128-row tiles; one 64-row half per warpgroup (H = 1), so that the promotion fragments of
+//         cluster_consume_tile_fp8 fit in the register file next to the accumulators.
+template <bool FP8>
+struct ClusterCfg {
+  static constexpr int H = FP8 ? 1 : 2;
+  static constexpr int BM = 128 * H;
+  static constexpr int BK = FP8 ? 128 : 64;
+  static constexpr int STAGES = FP8 ? 6 : 4;
+  static constexpr int A_BYTES = BM * 128;
+  static constexpr int B_BYTES = CBN * 128;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;
+};
+using Cfg16 = ClusterCfg<false>;
+using Cfg8 = ClusterCfg<true>;
+static_assert(Cfg16::BM == CBM && Cfg16::BK == BK, "bf16 cluster tile");
 
 // acc[h][64 x 128] (+)= rows [128 wg + 64 h, +64) of the stage's A box . W box^T, for one tile's K loop
 __device__ __forceinline__ void cluster_consume_tile(float (&acc)[2][64], uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
                                                      int num_kb, int wg, int& stage, uint32_t& phase) {
+  constexpr int C_STAGES = Cfg16::STAGES;
   const int lane = threadIdx.x & 31;
   int prev = -1;
   for (int kb = 0; kb < num_kb; ++kb) {
     mbar_wait(&full_bar[stage], phase);
-    const uint32_t sa = smem_u32(smem + stage * C_STAGE_BYTES);
+    const uint32_t sa = smem_u32(smem + stage * Cfg16::STAGE_BYTES);
     const uint64_t da0 = make_smem_desc_kmajor_sw128(sa + (2 * wg + 0) * (64 * 128));
     const uint64_t da1 = make_smem_desc_kmajor_sw128(sa + (2 * wg + 1) * (64 * 128));
-    const uint64_t db = make_smem_desc_kmajor_sw128(sa + C_A_BYTES);
+    const uint64_t db = make_smem_desc_kmajor_sw128(sa + Cfg16::A_BYTES);
     wgmma_reg_fence(acc[0]);
     wgmma_reg_fence(acc[1]);
     wgmma_fence();
@@ -366,17 +387,78 @@ __device__ __forceinline__ void cluster_consume_tile(float (&acc)[2][64], uint8_
   }
 }
 
+// t[64 x 128] = rows [64 wg, +64) of an e4m3 stage's A box . W box^T over the stage's K = 128 (four k32 steps), committed
+// as one wgmma group
+__device__ __forceinline__ void fp8_stage_mma(float (&t)[64], uint8_t* smem, int stage, int wg) {
+  const uint32_t sa = smem_u32(smem + stage * Cfg8::STAGE_BYTES);
+  const uint64_t da = make_smem_desc_kmajor_sw128(sa + wg * (64 * 128));
+  const uint64_t db = make_smem_desc_kmajor_sw128(sa + Cfg8::A_BYTES);
+  wgmma_reg_fence(t);
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < Cfg8::BK / 32; ++kk) wgmma_ss_n128_e4m3(t, da + 2 * kk, db + 2 * kk, kk != 0 ? 1u : 0u);
+  wgmma_commit();
+}
+
+// acc[0][64 x 128] = rows [64 wg, +64) of the tile, e4m3 operands.  Hopper's fp8 wgmma adds products into its accumulator
+// with reduced internal precision (about 14 bits), which over K = 9600 loses about 1e-2 relative.  So each stage (K = 128)
+// runs into a fresh fragment t, which is added into the fp32 accumulator with FADD once its group has retired (promotion);
+// the sum order depends on K only.  The fragment is read only after wait<0>: reading one while another group of the same
+// warpgroup is in flight makes ptxas serialise every wgmma (C7514).  The other consumer warpgroup's wgmmas fill the gap.
+__device__ __forceinline__ void cluster_consume_tile_fp8(float (&acc)[1][64], uint8_t* smem, uint64_t* full_bar,
+                                                         uint64_t* empty_bar, int num_kb, int wg, int& stage, uint32_t& phase) {
+  const int lane = threadIdx.x & 31;
+  float t[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[0][i] = 0.f;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    mbar_wait(&full_bar[stage], phase);
+    fp8_stage_mma(t, smem, stage, wg);
+    wgmma_wait<0>();
+    wgmma_reg_fence(t);
+    if (lane == 0) {
+      mbar_arrive_cluster(&empty_bar[stage], 0);
+      mbar_arrive_cluster(&empty_bar[stage], 1);
+    }
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[0][i] += t[i];
+    if (++stage == Cfg8::STAGES) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+}
+
 // Epilogue straight from the accumulator fragments (pf_common.cuh wgmma layout): thread (warp w, lane l) of consumer
-// warpgroup wg holds, for h, half in {0, 1}, tile row 128 wg + 64 h + 16 w + l / 4 + 8 half at columns 8 i + 2 (l % 4) + {0, 1},
-// i = 0..15, in acc[h][4 i + 2 half + {0, 1}].  Same arithmetic per element, in the same order, as the staged epilogue of the
-// 128-row kernels: the same bits.
-template <int EPI>
-__device__ __forceinline__ void epilogue_frag(const GemmArgs& g, const float (&acc)[2][64], int wg, int b, int m_base, int n_base) {
+// warpgroup wg holds, for h < H, half in {0, 1}, tile row 64 (H wg + h) + 16 w + l / 4 + 8 half at columns 8 i + 2 (l % 4)
+// + {0, 1}, i = 0..15, in acc[h][4 i + 2 half + {0, 1}].  Unscaled (bf16): same arithmetic per element, in the same order, as
+// the staged epilogue of the 128-row kernels: the same bits.  SCALED (e4m3): each accumulator is first multiplied by its
+// row's a_scale and then its column's w_scale; what follows is the same arithmetic.
+template <int EPI, int H, bool SCALED>
+__device__ __forceinline__ void epilogue_frag(const GemmArgs& g, const float (&acc)[H][64], int wg, int b, int m_base, int n_base) {
   const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-  const int r_thr = wg * 128 + w * 16 + (lane >> 2);   // + 64 h + 8 half
-  const int c_thr = 2 * (lane & 3);                    // + 8 i
+  const int r_thr = wg * 64 * H + w * 16 + (lane >> 2);   // + 64 h + 8 half
+  const int c_thr = 2 * (lane & 3);                       // + 8 i
   bool qkv_tile = (EPI == PF_EPI_QKV_ROPE);
   if (EPI == PF_EPI_QKV_GELU) qkv_tile = n_base < g.n_split;
+  float sa[2 * H];   // row scales of (h, half)
+  if constexpr (SCALED) {
+#pragma unroll
+    for (int hr = 0; hr < 2 * H; ++hr) {
+      const int m = m_base + r_thr + 64 * (hr >> 1) + 8 * (hr & 1);
+      sa[hr] = m < g.row_count ? __ldg(g.a_scale + static_cast<size_t>(b) * g.rows_per_batch + g.row_begin + m) : 0.f;
+    }
+  }
+  // the accumulator of (h, half) = hr at column n (n even): dequantised pair (n, n + 1)
+  auto value2 = [&](int hr, int idx, int n) -> float2 {
+    const float a0 = acc[hr >> 1][idx], a1 = acc[hr >> 1][idx + 1];
+    if constexpr (SCALED) {
+      const float2 ws = __ldg(reinterpret_cast<const float2*>(g.w_scale + n));
+      return make_float2(a0 * sa[hr] * ws.x, a1 * sa[hr] * ws.y);
+    } else {
+      return make_float2(a0, a1);
+    }
+  };
 
   if (qkv_tile) {
     const int inner = g.heads * g.head_dim;
@@ -388,7 +470,7 @@ __device__ __forceinline__ void epilogue_frag(const GemmArgs& g, const float (&a
       __nv_bfloat16* base = section == 0 ? g.q_out : (section == 1 ? g.k_out : g.v_out);
       const float* nw = section == 0 ? g.q_norm_w : g.k_norm_w;
 #pragma unroll
-      for (int hr = 0; hr < 4; ++hr) {
+      for (int hr = 0; hr < 2 * H; ++hr) {
         const int h = hr >> 1, half = hr & 1;
         const int m = m_base + r_thr + 64 * h + 8 * half;
         const bool valid = m < g.row_count;
@@ -398,8 +480,9 @@ __device__ __forceinline__ void epilogue_frag(const GemmArgs& g, const float (&a
         for (int j = 0; j < 8; ++j) {
           float2 bb = make_float2(0.f, 0.f);
           if (g.bias != nullptr) bb = __ldg(reinterpret_cast<const float2*>(g.bias + n0 + 8 * j + c_thr));
-          x[2 * j + 0] = acc[h][4 * (8 * hh + j) + 2 * half + 0] + bb.x;
-          x[2 * j + 1] = acc[h][4 * (8 * hh + j) + 2 * half + 1] + bb.y;
+          const float2 a = value2(hr, 4 * (8 * hh + j) + 2 * half, n0 + 8 * j + c_thr);
+          x[2 * j + 0] = a.x + bb.x;
+          x[2 * j + 1] = a.y + bb.y;
         }
         if (section < 2) {   // RMSNorm over the head (N:66-79), then RoPE (B:34-39)
           // The staged epilogue's sum order: chain c (0..3) runs over columns 4 k + c, k ascending, and the head's sum is
@@ -457,7 +540,7 @@ __device__ __forceinline__ void epilogue_frag(const GemmArgs& g, const float (&a
     const float* gate = g.gate + b * g.gate_batch_stride + n_base + c_thr;
     float* obase = reinterpret_cast<float*>(g.out) + g.out_col_begin + n_base + c_thr;
 #pragma unroll
-    for (int hr = 0; hr < 4; ++hr) {
+    for (int hr = 0; hr < 2 * H; ++hr) {
       const int h = hr >> 1, half = hr & 1;
       const int m = m_base + r_thr + 64 * h + 8 * half;
       if (m >= g.row_count) continue;
@@ -470,8 +553,9 @@ __device__ __forceinline__ void epilogue_frag(const GemmArgs& g, const float (&a
         float2 bb = make_float2(0.f, 0.f);
         if (g.bias != nullptr) bb = __ldg(reinterpret_cast<const float2*>(g.bias + n_base + 8 * i + c_thr));
         const float2 gg = __ldg(reinterpret_cast<const float2*>(gate + 8 * i));
-        const float x0 = acc[h][4 * i + 2 * half + 0] + bb.x;
-        const float x1 = acc[h][4 * i + 2 * half + 1] + bb.y;
+        const float2 a = value2(hr, 4 * i + 2 * half, n_base + 8 * i + c_thr);
+        const float x0 = a.x + bb.x;
+        const float x1 = a.y + bb.y;
         rr[i].x += gg.x * x0;
         rr[i].y += gg.y * x1;
         dst[4 * i] = rr[i];
@@ -484,11 +568,12 @@ __device__ __forceinline__ void epilogue_frag(const GemmArgs& g, const float (&a
       float2 bb = make_float2(0.f, 0.f);
       if (g.bias != nullptr) bb = __ldg(reinterpret_cast<const float2*>(g.bias + n));
 #pragma unroll
-      for (int hr = 0; hr < 4; ++hr) {
+      for (int hr = 0; hr < 2 * H; ++hr) {
         const int h = hr >> 1, half = hr & 1;
         const int m = m_base + r_thr + 64 * h + 8 * half;
-        float x0 = acc[h][4 * i + 2 * half + 0] + bb.x;
-        float x1 = acc[h][4 * i + 2 * half + 1] + bb.y;
+        const float2 a = value2(hr, 4 * i + 2 * half, n);
+        float x0 = a.x + bb.x;
+        float x1 = a.y + bb.y;
         if (EPI == PF_EPI_GELU_BF16 || EPI == PF_EPI_QKV_GELU) {
           x0 = gelu_tanh_f(x0);
           x1 = gelu_tanh_f(x1);
@@ -506,10 +591,11 @@ __device__ __forceinline__ void epilogue_frag(const GemmArgs& g, const float (&a
   }
 }
 
-template <int EPI>
+template <int EPI, bool FP8>
 __global__ void __launch_bounds__(PIPE_THREADS, 1)
-gemm_bf16_cluster_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
-                         const GemmArgs g) {
+gemm_cluster_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b, const GemmArgs g) {
+  using Cfg = ClusterCfg<FP8>;
+  constexpr int C_STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
@@ -535,7 +621,7 @@ gemm_bf16_cluster_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_
 
   // Static schedule over tile pairs: both CTAs of a cluster walk the same pairs.  m_tiles is even-padded per batch; the
   // partner of an odd last tile loads rows past row_count (zero-filled or masked) and stores nothing.
-  const int num_kb = (g.k + BK - 1) / BK;
+  const int num_kb = (g.k + Cfg::BK - 1) / Cfg::BK;
   const int m_pairs = (g.m_tiles + 1) >> 1;
   const int pairs_per_batch = m_pairs * g.n_tiles;
   const int total_pairs = g.batches * pairs_per_batch;
@@ -554,10 +640,10 @@ gemm_bf16_cluster_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_
         const int nt = r % g.n_tiles;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * C_STAGE_BYTES;
-          mbar_arrive_expect_tx(&full_bar[stage], C_STAGE_BYTES);
-          tma_load_3d(sa, &tm_a, &full_bar[stage], kb * BK, g.row_begin + mt * CBM, b);
-          tma_load_2d_multicast(sa + C_A_BYTES + rank * (C_B_BYTES / 2), &tm_b, &full_bar[stage], kb * BK,
+          uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
+          mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+          tma_load_3d(sa, &tm_a, &full_bar[stage], kb * Cfg::BK, g.row_begin + mt * Cfg::BM, b);
+          tma_load_2d_multicast(sa + Cfg::A_BYTES + rank * (Cfg::B_BYTES / 2), &tm_b, &full_bar[stage], kb * Cfg::BK,
                                 nt * CBN + rank * (CBN / 2), 0x3);
           if (++stage == C_STAGES) {
             stage = 0;
@@ -568,19 +654,20 @@ gemm_bf16_cluster_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_
     }
     __syncwarp();
   } else {
-    // ===== consumers: each warpgroup owns 128 rows of the tile =====
+    // ===== consumers: each warpgroup owns 64 H rows of the tile =====
     setmaxnreg_inc<232>();
     const int wg = wgroup - 1;
     int stage = 0;
     uint32_t phase = 0;
-    float acc[2][64];
+    float acc[Cfg::H][64];
     for (int p = cluster; p < total_pairs; p += clusters) {
       const int b = p / pairs_per_batch;
       const int r = p - b * pairs_per_batch;
       const int mt = 2 * (r / g.n_tiles) + static_cast<int>(rank);
       const int nt = r % g.n_tiles;
-      cluster_consume_tile(acc, smem, full_bar, empty_bar, num_kb, wg, stage, phase);
-      epilogue_frag<EPI>(g, acc, wg, b, mt * CBM, nt * CBN);
+      if constexpr (FP8) cluster_consume_tile_fp8(acc, smem, full_bar, empty_bar, num_kb, wg, stage, phase);
+      else cluster_consume_tile(acc, smem, full_bar, empty_bar, num_kb, wg, stage, phase);
+      epilogue_frag<EPI, Cfg::H, FP8>(g, acc, wg, b, mt * Cfg::BM, nt * CBN);
     }
   }
   // no CTA exits while its peer may still arrive on its barriers
@@ -601,14 +688,16 @@ static int launch_gemm(const CUtensorMap& tm_a, const CUtensorMap& tm_b, const G
   return check_launch("pf_gemm_bf16");
 }
 
-// Clusters of the 256 x 128 kernel that fit on the device at once (SMs pair up within a GPC, so this can be below
-// num_sms() / 2); queried once, before any CUDA-graph capture, by warmup_gemm.
+// Clusters of the cluster kernel that fit on the device at once (SMs pair up within a GPC, so this can be below
+// num_sms() / 2); queried once, before any CUDA-graph capture, by warmup_gemm.  Both operand types take one CTA per SM and
+// the same shared memory.
+static_assert(Cfg8::SMEM_BYTES == Cfg16::SMEM_BYTES, "one cluster occupancy for both operand types");
 static int g_cluster_slots = 0;
 
 static int cluster_slots() {
   if (g_cluster_slots > 0) return g_cluster_slots;
-  auto kern = gemm_bf16_cluster_kernel<PF_EPI_STORE_BF16>;
-  if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), C_SMEM_BYTES, "gemm cluster")) return rc;
+  auto kern = gemm_cluster_kernel<PF_EPI_STORE_BF16, false>;
+  if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), Cfg16::SMEM_BYTES, "gemm cluster")) return rc;
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -617,7 +706,7 @@ static int cluster_slots() {
   attr[0].val.clusterDim.z = 1;
   cfg.gridDim = dim3(2, 1, 1);
   cfg.blockDim = dim3(PIPE_THREADS, 1, 1);
-  cfg.dynamicSmemBytes = C_SMEM_BYTES;
+  cfg.dynamicSmemBytes = Cfg16::SMEM_BYTES;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   int n = 0;
@@ -629,10 +718,11 @@ static int cluster_slots() {
   return n;
 }
 
-template <int EPI>
+template <int EPI, bool FP8 = false>
 static int launch_cluster(const CUtensorMap& tm_a, const CUtensorMap& tm_b, const GemmArgs& g, cudaStream_t stream) {
-  auto kern = gemm_bf16_cluster_kernel<EPI>;
-  if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), C_SMEM_BYTES, "gemm cluster")) return rc;
+  auto kern = gemm_cluster_kernel<EPI, FP8>;
+  constexpr int smem_bytes = ClusterCfg<FP8>::SMEM_BYTES;
+  if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(kern), smem_bytes, "gemm cluster")) return rc;
   const int slots = cluster_slots();
   if (slots < 0) return slots;
   const int pairs = g.batches * ((g.m_tiles + 1) / 2) * g.n_tiles;
@@ -644,12 +734,12 @@ static int launch_cluster(const CUtensorMap& tm_a, const CUtensorMap& tm_b, cons
   attr[0].val.clusterDim.z = 1;
   cfg.gridDim = dim3(2 * (pairs < slots ? pairs : slots), 1, 1);
   cfg.blockDim = dim3(PIPE_THREADS, 1, 1);
-  cfg.dynamicSmemBytes = C_SMEM_BYTES;
+  cfg.dynamicSmemBytes = smem_bytes;
   cfg.stream = stream;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   (void)cudaLaunchKernelEx(&cfg, kern, tm_a, tm_b, g);
-  return check_launch("pf_gemm_bf16");
+  return check_launch(FP8 ? "pf_gemm_fp8" : "pf_gemm_bf16");
 }
 
 // tile 0 = 256 x 128 in 2-CTA clusters, else the 128-row kernel with BLOCK_N = tile
@@ -666,7 +756,8 @@ static int dispatch_tile(int tile, const CUtensorMap& tm_a, const CUtensorMap& t
 
 template <int EPI>
 static int warm_epi() {
-  int rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_bf16_cluster_kernel<EPI>), C_SMEM_BYTES, "gemm cluster");
+  int rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_cluster_kernel<EPI, false>), Cfg16::SMEM_BYTES, "gemm cluster");
+  if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_cluster_kernel<EPI, true>), Cfg8::SMEM_BYTES, "gemm cluster fp8");
   if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_bf16_wgmma_kernel<128, EPI>), PipeCfg<128>::SMEM_BYTES, "gemm<128>");
   if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_bf16_wgmma_kernel<64, EPI>), PipeCfg<64>::SMEM_BYTES, "gemm<64>");
   return rc;
@@ -684,53 +775,47 @@ int warmup_gemm() {
   return rc;
 }
 
-}  // namespace pf
-
-extern "C" int pf_gemm_bf16(const pf_gemm_desc* d, void* stream_) {
-  using namespace pf;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  PF_REQUIRE(d != nullptr, "pf_gemm_bf16: null descriptor");
-  PF_REQUIRE(d->a && d->w, "pf_gemm_bf16: null operand");
-  PF_REQUIRE(d->k > 0 && d->k % 8 == 0, "pf_gemm_bf16: k=%d must be a positive multiple of 8", d->k);
-  PF_REQUIRE(d->lda % 8 == 0 && d->lda >= d->k, "pf_gemm_bf16: lda=%lld must be >= k and a multiple of 8", (long long)d->lda);
+// Validation shared by both entries (everything except the operand format), then the kernel arguments from the descriptor.
+// `fn` names the entry in the messages; `k_align` = elements per 16 bytes of A / W (TMA row strides).
+static int gemm_args_from_desc(const pf_gemm_desc* d, const char* fn, int k_align, GemmArgs& g) {
+  PF_REQUIRE(d->a && d->w, "%s: null operand", fn);
+  PF_REQUIRE(d->k > 0 && d->k % k_align == 0, "%s: k=%d must be a positive multiple of %d", fn, d->k, k_align);
+  PF_REQUIRE(d->lda % k_align == 0 && d->lda >= d->k, "%s: lda=%lld must be >= k and a multiple of %d", fn, (long long)d->lda,
+             k_align);
   PF_REQUIRE(d->batches > 0 && d->rows_per_batch > 0 && d->row_count > 0 && d->row_begin >= 0 &&
                  d->row_begin + d->row_count <= d->rows_per_batch,
-             "pf_gemm_bf16: bad row range (batches %d rows %d begin %d count %d)", d->batches, d->rows_per_batch,
+             "%s: bad row range (batches %d rows %d begin %d count %d)", fn, d->batches, d->rows_per_batch,
              d->row_begin, d->row_count);
   PF_REQUIRE((reinterpret_cast<uintptr_t>(d->a) & 15) == 0 && (reinterpret_cast<uintptr_t>(d->w) & 15) == 0,
-             "pf_gemm_bf16: operands must be 16-byte aligned");
+             "%s: operands must be 16-byte aligned", fn);
   const int epi = d->epilogue;
-  PF_REQUIRE(epi >= 0 && epi <= PF_EPI_QKV_GELU, "pf_gemm_bf16: unknown epilogue %d", epi);
+  PF_REQUIRE(epi >= 0 && epi <= PF_EPI_QKV_GELU, "%s: unknown epilogue %d", fn, epi);
 
-  // Column tiling: 128-wide tiles when they divide n, else 64-wide.  The QKV epilogues work per 64-column head, so any
-  // multiple of 64 is head-aligned.
-  int bn = 0;
+  // The QKV epilogues work per 64-column head, so any multiple of 64 is head-aligned.
   const bool qkv = (epi == PF_EPI_QKV_ROPE || epi == PF_EPI_QKV_GELU);
   if (qkv) {
-    PF_REQUIRE(d->head_dim == 64, "pf_gemm_bf16: QKV epilogue supports head_dim 64 only (got %d)", d->head_dim);
+    PF_REQUIRE(d->head_dim == 64, "%s: QKV epilogue supports head_dim 64 only (got %d)", fn, d->head_dim);
     const int inner = d->heads * d->head_dim;
     const int nq = 3 * inner;
-    PF_REQUIRE(d->q_out && d->k_out && d->v_out && d->q_norm_w && d->k_norm_w, "pf_gemm_bf16: QKV epilogue needs q/k/v outputs and norm weights");
-    PF_REQUIRE(d->out_row_begin + d->row_count <= d->seq_len, "pf_gemm_bf16: QKV rows exceed seq_len");
+    PF_REQUIRE(d->q_out && d->k_out && d->v_out && d->q_norm_w && d->k_norm_w, "%s: QKV epilogue needs q/k/v outputs and norm weights", fn);
+    PF_REQUIRE(d->out_row_begin + d->row_count <= d->seq_len, "%s: QKV rows exceed seq_len", fn);
     if (epi == PF_EPI_QKV_ROPE) {
-      PF_REQUIRE(d->n == nq, "pf_gemm_bf16: QKV_ROPE needs n == 3*heads*head_dim");
+      PF_REQUIRE(d->n == nq, "%s: QKV_ROPE needs n == 3*heads*head_dim", fn);
     } else {
-      PF_REQUIRE(d->n_split == nq && d->n > nq && d->out != nullptr, "pf_gemm_bf16: QKV_GELU needs n_split == 3*heads*head_dim < n and out");
-      PF_REQUIRE(nq % 64 == 0, "pf_gemm_bf16: n_split must be a multiple of 64");
+      PF_REQUIRE(d->n_split == nq && d->n > nq && d->out != nullptr, "%s: QKV_GELU needs n_split == 3*heads*head_dim < n and out", fn);
+      PF_REQUIRE(nq % 64 == 0, "%s: n_split must be a multiple of 64", fn);
     }
   } else {
-    PF_REQUIRE(d->out != nullptr, "pf_gemm_bf16: null output");
-    if (epi == PF_EPI_GATE_RESID) PF_REQUIRE(d->gate != nullptr, "pf_gemm_bf16: GATE_RESID needs gate");
+    PF_REQUIRE(d->out != nullptr, "%s: null output", fn);
+    if (epi == PF_EPI_GATE_RESID) PF_REQUIRE(d->gate != nullptr, "%s: GATE_RESID needs gate", fn);
     const int esz = (epi == PF_EPI_STORE_F32 || epi == PF_EPI_GATE_RESID) ? 4 : 2;
     PF_REQUIRE((d->ldo * esz) % 16 == 0 && (d->out_col_begin * esz) % 16 == 0 &&
                    (reinterpret_cast<uintptr_t>(d->out) & 15) == 0,
-               "pf_gemm_bf16: output must be 16-byte aligned (ldo %lld col %d)", (long long)d->ldo, d->out_col_begin);
+               "%s: output must be 16-byte aligned (ldo %lld col %d)", fn, (long long)d->ldo, d->out_col_begin);
   }
-  PF_REQUIRE(d->n % 64 == 0, "pf_gemm_bf16: n=%d must be a multiple of 64", d->n);
-  // QKV_GELU: tiles must not straddle the q|k|v / mlp boundary (different epilogue per tile)
-  bn = (d->n % 128 == 0 && (epi != PF_EPI_QKV_GELU || d->n_split % 128 == 0)) ? 128 : 64;
+  PF_REQUIRE(d->n % 64 == 0, "%s: n=%d must be a multiple of 64", fn, d->n);
 
-  GemmArgs g{};
+  g = GemmArgs{};
   g.batches = d->batches;
   g.row_begin = d->row_begin;
   g.row_count = d->row_count;
@@ -760,14 +845,30 @@ extern "C" int pf_gemm_bf16(const pf_gemm_desc* d, void* stream_) {
   g.peer_heads = d->peer_heads;
   g.peer_seq = d->peer_seq;
   g.peer_row0 = d->peer_row0;
+  g.rows_per_batch = d->rows_per_batch;
   for (int i = 0; i < PF_MAX_PEERS; ++i) g.peer_qkv[i] = static_cast<__nv_bfloat16*>(d->peer_qkv[i]);
   if (d->peer_count > 1) {
-    PF_REQUIRE(epi == PF_EPI_QKV_ROPE && d->batches == 1, "pf_gemm_bf16: peer stores need the QKV_ROPE epilogue and batches == 1");
+    PF_REQUIRE(epi == PF_EPI_QKV_ROPE && d->batches == 1, "%s: peer stores need the QKV_ROPE epilogue and batches == 1", fn);
     PF_REQUIRE(d->peer_count <= PF_MAX_PEERS && d->peer_heads > 0 && d->peer_heads * d->peer_count >= d->heads &&
                    d->peer_row0 >= 0 && d->peer_row0 + d->out_row_begin + d->row_count <= d->peer_seq,
-               "pf_gemm_bf16: bad peer layout (count %d heads/rank %d seq %d row0 %d)", d->peer_count, d->peer_heads, d->peer_seq, d->peer_row0);
-    for (int i = 0; i < d->peer_count; ++i) PF_REQUIRE(d->peer_qkv[i] != nullptr, "pf_gemm_bf16: peer_qkv[%d] is null", i);
+               "%s: bad peer layout (count %d heads/rank %d seq %d row0 %d)", fn, d->peer_count, d->peer_heads, d->peer_seq, d->peer_row0);
+    for (int i = 0; i < d->peer_count; ++i) PF_REQUIRE(d->peer_qkv[i] != nullptr, "%s: peer_qkv[%d] is null", fn, i);
   }
+  return 0;
+}
+
+}  // namespace pf
+
+extern "C" int pf_gemm_bf16(const pf_gemm_desc* d, void* stream_) {
+  using namespace pf;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  PF_REQUIRE(d != nullptr, "pf_gemm_bf16: null descriptor");
+  GemmArgs g;
+  if (int rc = gemm_args_from_desc(d, "pf_gemm_bf16", 8, g)) return rc;
+  const int epi = d->epilogue;
+  // Column tiling: 128-wide tiles when they divide n, else 64-wide.
+  // QKV_GELU: tiles must not straddle the q|k|v / mlp boundary (different epilogue per tile)
+  int bn = (d->n % 128 == 0 && (epi != PF_EPI_QKV_GELU || d->n_split % 128 == 0)) ? 128 : 64;
 
   // Kernels: tile 0 = 256 x 128 in 2-CTA clusters (needs 128 | n), 128 = 128 x 128, 64 = 128 x 64.  All three run the same
   // wgmma k16 steps in the same order per output element and the same epilogue arithmetic: same bits whichever runs.
@@ -823,6 +924,49 @@ extern "C" int pf_gemm_bf16(const pf_gemm_desc* d, void* stream_) {
     case PF_EPI_GATE_RESID: return dispatch_tile<PF_EPI_GATE_RESID>(tile, tm_a, tm_b, g, stream);
     case PF_EPI_QKV_ROPE: return dispatch_tile<PF_EPI_QKV_ROPE>(tile, tm_a, tm_b, g, stream);
     case PF_EPI_QKV_GELU: return dispatch_tile<PF_EPI_QKV_GELU>(tile, tm_a, tm_b, g, stream);
+  }
+  return -1;
+}
+
+extern "C" int pf_gemm_fp8(const pf_gemm_desc* d, const float* a_row_scale, const float* w_col_scale, void* stream_) {
+  using namespace pf;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  PF_REQUIRE(d != nullptr, "pf_gemm_fp8: null descriptor");
+  PF_REQUIRE(a_row_scale != nullptr && w_col_scale != nullptr, "pf_gemm_fp8: null scale (a_row_scale and w_col_scale are required)");
+  PF_REQUIRE(d->peer_count <= 0, "pf_gemm_fp8: sequence-parallel peer stores (peer_count %d) are bf16 only", d->peer_count);
+  PF_REQUIRE(d->kernel_variant == 0, "pf_gemm_fp8: kernel_variant %d: there is one fp8 kernel (0)", d->kernel_variant);
+  PF_REQUIRE(d->n % 128 == 0, "pf_gemm_fp8: n=%d must be a multiple of 128", d->n);
+  PF_REQUIRE(d->epilogue != PF_EPI_QKV_GELU || d->n_split % 128 == 0, "pf_gemm_fp8: QKV_GELU needs n_split %% 128 == 0");
+  GemmArgs g;
+  if (int rc = gemm_args_from_desc(d, "pf_gemm_fp8", 16, g)) return rc;
+  g.a_scale = a_row_scale;
+  g.w_scale = w_col_scale;
+  g.m_tiles = (d->row_count + Cfg8::BM - 1) / Cfg8::BM;
+  g.n_tiles = d->n / CBN;
+  CUtensorMap tm_a, tm_b;
+  {
+    const uint64_t dims[3] = {static_cast<uint64_t>(d->k), static_cast<uint64_t>(d->rows_per_batch),
+                              static_cast<uint64_t>(d->batches)};
+    const uint64_t strides[2] = {static_cast<uint64_t>(d->lda),
+                                 static_cast<uint64_t>(d->lda) * static_cast<uint64_t>(d->rows_per_batch)};
+    const uint32_t box[3] = {Cfg8::BK, Cfg8::BM, 1};
+    if (int rc = encode_tensor_map(&tm_a, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, d->a, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))
+      return rc;
+  }
+  {
+    const uint64_t dims[2] = {static_cast<uint64_t>(d->k), static_cast<uint64_t>(d->n)};
+    const uint64_t strides[1] = {static_cast<uint64_t>(d->k)};
+    const uint32_t box[2] = {Cfg8::BK, CBN / 2};   // each CTA of the cluster loads half of the W box
+    if (int rc = encode_tensor_map(&tm_b, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, d->w, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))
+      return rc;
+  }
+  switch (d->epilogue) {
+    case PF_EPI_STORE_BF16: return launch_cluster<PF_EPI_STORE_BF16, true>(tm_a, tm_b, g, stream);
+    case PF_EPI_GELU_BF16: return launch_cluster<PF_EPI_GELU_BF16, true>(tm_a, tm_b, g, stream);
+    case PF_EPI_STORE_F32: return launch_cluster<PF_EPI_STORE_F32, true>(tm_a, tm_b, g, stream);
+    case PF_EPI_GATE_RESID: return launch_cluster<PF_EPI_GATE_RESID, true>(tm_a, tm_b, g, stream);
+    case PF_EPI_QKV_ROPE: return launch_cluster<PF_EPI_QKV_ROPE, true>(tm_a, tm_b, g, stream);
+    case PF_EPI_QKV_GELU: return launch_cluster<PF_EPI_QKV_GELU, true>(tm_a, tm_b, g, stream);
   }
   return -1;
 }

@@ -14,6 +14,12 @@ stream (no torch math on the path, no CPU fallback):
   16 x single block: LN+modulate | QKV GEMM (+RMSNorm, RoPE) | proj_mlp GEMM (+GELU) | attention | proj_out GEMM over [attn|mlp]
   head             : LN+modulate (last-frame tokens only) | proj_out GEMM | unpatchify
 
+gemm_precision="fp8" (opt-in, changes the numerics; include/pf_b200.h FP8 contract): the video-range QKV, to_out, FF1 and FF2
+GEMMs of the double blocks and all three GEMMs of every single block run on e4m3 operands (per-token activation scales,
+per-output-channel weight scales quantised once at import).  Their A operands come from the quantising LN-modulate or from
+a row quantiser pass over `cat` (timer tag "quantize_fp8").  The text stream of the double blocks, the embedders, the head
+and the conditioning / AdaLN GEMVs stay bf16.
+
 Data layout in HBM (B = CFG batch, S = text + all clip tokens, D = heads*64):
   h    fp32 [B, S, D]      joint residual stream ([text ; clip_0 ; ... ; clip_n] per sample) — fp32 so that 48 residual
                            adds do not accumulate bf16 rounding (the reference keeps it bf16)
@@ -21,6 +27,10 @@ Data layout in HBM (B = CFG batch, S = text + all clip tokens, D = heads*64):
   q,k,v bf16 [B, H, S, 64] head-major, written by the QKV epilogue, read by TMA in the attention kernel
   cat  bf16 [B, S, 5D]     [attention out | MLP hidden] — proj_out of the single block reads it without a concat copy
   mod  fp32 [B, N_mod]     every layer's (shift, scale, gate, ...) from ONE GEMV per step
+  fp8 only:
+  xn8  e4m3 [B, S, 5D]     twin of `cat`: quantised [attention out | MLP hidden] rows; its first B*S*D bytes also hold the
+                           LN-modulate output [B, S, D] (consumed by QKV / FF1 / proj_mlp before the twin is refilled)
+  sx8, sc8 fp32 [B, S]     row scales of the LN-modulate output and of the quantised `cat` rows
 """
 from __future__ import annotations
 
@@ -178,8 +188,12 @@ class B200FluxTransformer(torch.nn.Module):
     """Holder of packed bf16 weights + the kernel-launch sequence of one DiT step."""
 
     def __init__(self, config: FluxConfigB200, state_dict: Dict[str, torch.Tensor], device="cuda",
-                 emulate_bf16_rounding: bool = False):
+                 emulate_bf16_rounding: bool = False, gemm_precision: str = "bf16"):
         super().__init__()
+        if gemm_precision not in ("bf16", "fp8"):
+            raise ValueError(f"gemm_precision must be 'bf16' or 'fp8', not {gemm_precision!r}")
+        # "fp8": the block GEMMs listed in the module docstring run on e4m3 operands (opt-in: different numerics)
+        self.gemm_precision = gemm_precision
         self.cfg = config
         # True reproduces the reference's bf16 rounding of the sinusoidal projection (E:195); False keeps fp32
         self.emulate_bf16_rounding = emulate_bf16_rounding
@@ -235,6 +249,15 @@ class B200FluxTransformer(torch.nn.Module):
         def V(name):
             return sd[name].float().to(device).contiguous()
 
+        fp8 = self.gemm_precision == "fp8"
+
+        def WQ(blk, key, *names):   # the weight of a GEMM that runs in fp8 under gemm_precision="fp8"
+            if fp8:                 # e4m3 [N, K] + fp32 per-channel scale "s_..." from the fp32 values (host), no bf16 copy
+                w8, sc = ops.quantize_weight_fp8(torch.cat([sd[n + ".weight"].float().cpu() for n in names], 0))
+                blk[key], blk["s" + key[1:]] = w8.to(device), sc.to(device)
+            else:
+                blk[key] = W(*names)
+
         reg = self.register_buffer
         reg("w_t1", W("time_text_embed.timestep_embedder.linear_1")); reg("b_t1", Bv("time_text_embed.timestep_embedder.linear_1"))
         reg("w_t2", W("time_text_embed.timestep_embedder.linear_2")); reg("b_t2", Bv("time_text_embed.timestep_embedder.linear_2"))
@@ -261,31 +284,36 @@ class B200FluxTransformer(torch.nn.Module):
         for i in range(c.num_layers):
             p = f"transformer_blocks.{i}"
             blk = dict(
-                w_qkv=W(p + ".attn.to_q", p + ".attn.to_k", p + ".attn.to_v"),
                 b_qkv=Bv(p + ".attn.to_q", p + ".attn.to_k", p + ".attn.to_v"),
                 w_cqkv=W(p + ".attn.add_q_proj", p + ".attn.add_k_proj", p + ".attn.add_v_proj"),
                 b_cqkv=Bv(p + ".attn.add_q_proj", p + ".attn.add_k_proj", p + ".attn.add_v_proj"),
                 nq=V(p + ".attn.norm_q.weight"), nk=V(p + ".attn.norm_k.weight"),
                 cnq=V(p + ".attn.norm_added_q.weight"), cnk=V(p + ".attn.norm_added_k.weight"),
-                w_o=W(p + ".attn.to_out.0"), b_o=Bv(p + ".attn.to_out.0"),
+                b_o=Bv(p + ".attn.to_out.0"),
                 w_co=W(p + ".attn.to_add_out"), b_co=Bv(p + ".attn.to_add_out"),
-                w_f1=W(p + ".ff.net.0.proj"), b_f1=Bv(p + ".ff.net.0.proj"),
-                w_f2=W(p + ".ff.net.2"), b_f2=Bv(p + ".ff.net.2"),
+                b_f1=Bv(p + ".ff.net.0.proj"),
+                b_f2=Bv(p + ".ff.net.2"),
                 w_cf1=W(p + ".ff_context.net.0.proj"), b_cf1=Bv(p + ".ff_context.net.0.proj"),
                 w_cf2=W(p + ".ff_context.net.2"), b_cf2=Bv(p + ".ff_context.net.2"),
             )
+            WQ(blk, "w_qkv", p + ".attn.to_q", p + ".attn.to_k", p + ".attn.to_v")
+            WQ(blk, "w_o", p + ".attn.to_out.0")
+            WQ(blk, "w_f1", p + ".ff.net.0.proj")
+            WQ(blk, "w_f2", p + ".ff.net.2")
             for k2, v2 in blk.items():
                 reg(f"dbl{i}_{k2}", v2)
             self.dbl.append(blk)
         for i in range(c.num_single_layers):
             p = f"single_transformer_blocks.{i}"
             blk = dict(
-                w_qkv=W(p + ".attn.to_q", p + ".attn.to_k", p + ".attn.to_v"),
                 b_qkv=Bv(p + ".attn.to_q", p + ".attn.to_k", p + ".attn.to_v"),
-                w_mlp=W(p + ".proj_mlp"), b_mlp=Bv(p + ".proj_mlp"),
+                b_mlp=Bv(p + ".proj_mlp"),
                 nq=V(p + ".attn.norm_q.weight"), nk=V(p + ".attn.norm_k.weight"),
-                w_out=W(p + ".proj_out"), b_out=Bv(p + ".proj_out"),
+                b_out=Bv(p + ".proj_out"),
             )
+            WQ(blk, "w_qkv", p + ".attn.to_q", p + ".attn.to_k", p + ".attn.to_v")
+            WQ(blk, "w_mlp", p + ".proj_mlp")
+            WQ(blk, "w_out", p + ".proj_out")
             for k2, v2 in blk.items():
                 reg(f"sgl{i}_{k2}", v2)
             self.sgl.append(blk)
@@ -326,6 +354,10 @@ class B200FluxTransformer(torch.nn.Module):
                 tmp=torch.empty(b, d, device=dev, dtype=torch.float32),
                 head=torch.zeros(b, plan.last_tokens, c.in_channels, device=dev, dtype=torch.float32),
             )
+            if self.gemm_precision == "fp8":
+                ws["xn8"] = torch.empty(b, sl, hp * 64 + 4 * d, device=dev, dtype=torch.float8_e4m3fn)
+                ws["sx8"] = torch.empty(b, sl, device=dev, dtype=torch.float32)
+                ws["sc8"] = torch.empty(b, sl, device=dev, dtype=torch.float32)
             if sl != plan.seq:   # sequence parallel: attention output of my head group over the whole sequence
                 lay = self.layout
                 ws["of"] = torch.empty(plan.seq, (hp // lay.sp) * 64, device=dev, dtype=torch.bfloat16)
@@ -360,6 +392,9 @@ class B200FluxTransformer(torch.nn.Module):
         exchange = "peer": q/k/v and the attention output cross NVLink as remote stores fused into the QKV GEMM / attention
         epilogues + flag barriers (csrc/pf_peer.cu): no NCCL call in the step, CUDA-graph capturable.  "nccl": the
         all_to_all_single formulation (kept for A/B measurements)."""
+        if self.gemm_precision == "fp8":
+            raise NotImplementedError("gemm_precision='fp8' runs on one GPU only: the sequence-parallel peer-store epilogues "
+                                      "have no fp8 form (build the model with gemm_precision='bf16' for a parallel layout)")
         assert exchange in ("peer", "nccl")
         if layout.sp > 1:   # see _lib.load(): one attention kernel for the whole process once sequence parallelism is in play
             _lib.set_option(_lib.PF_OPT_ATTN_TRIPLE_KERNEL, 0)
@@ -545,6 +580,21 @@ class B200FluxTransformer(torch.nn.Module):
                     ops.ln_modulate(h, xn, mod[:, off_shift:], mod[:, off_scale:], nm, batches=b, rows_per_batch=sl,
                                     row_begin=r0, row_count=rc)
 
+        fp8 = self.gemm_precision == "fp8"
+        if fp8:
+            xn8, sx8, sc8 = ws["xn8"], ws["sx8"], ws["sc8"]
+            xa8 = xn8.view(-1)[:b * sl * d].view(b, sl, d)    # LN-modulate output, row stride d (module docstring)
+
+        def lnmod8(off_shift, off_scale, r0, rc):
+            with T("ln_modulate"):
+                ops.ln_modulate_fp8(h, xa8, sx8, mod[:, off_shift:], mod[:, off_scale:], nm, batches=b, rows_per_batch=sl,
+                                    row_begin=r0, row_count=rc)
+
+        def quant8(col0, col1, r0, rc):   # cat[:, r0:r0 + rc, col0:col1] -> the same block of xn8, row scales -> sc8
+            with T("quantize_fp8"):
+                ops.quantize_rows_fp8(cat[:, :, col0:col1], xn8[:, :, col0:col1], sc8, batches=b, rows_per_batch=sl,
+                                      row_begin=r0, row_count=rc)
+
         peer_qkv = None
         if px is not None and nsp > 1:
             # QKV epilogue stores head h of my rows into rank (h // Hg)'s gathered buffer at sequence position c0 + row
@@ -556,6 +606,12 @@ class B200FluxTransformer(torch.nn.Module):
                     ops.gemm(xn, wq, bq, PF_EPI_QKV_ROPE, batches=b, rows_per_batch=sl, row_begin=r0, row_count=rc,
                              q_out=q, k_out=k, v_out=v, rope=rope, q_norm_w=nq, k_norm_w=nk, heads=hn, head_dim=64,
                              seq_len=sl, peer=peer_qkv)
+
+        def qkv8(wq, sq, bq, nq, nk, r0, rc):
+            with T("gemm_qkv"):
+                ops.gemm_fp8(xa8, sx8, wq, sq, bq, PF_EPI_QKV_ROPE, batches=b, rows_per_batch=sl, row_begin=r0, row_count=rc,
+                             q_out=q, k_out=k, v_out=v, rope=rope, q_norm_w=nq, k_norm_w=nk, heads=hn, head_dim=64,
+                             seq_len=sl)
 
         scale = 1.0 / math.sqrt(64)
         seg, tim, sched, sched2 = plan.seg[b0:b0 + b], plan.time[b0:b0 + b], plan.sched[b0:b0 + b], plan.sched2[b0:b0 + b]
@@ -614,11 +670,30 @@ class B200FluxTransformer(torch.nn.Module):
             wf1, bf1 = (w["w_cf1"], w["w_f1"]), (w["b_cf1"], w["b_f1"])
             wf2, bf2 = (w["w_cf2"], w["w_f2"]), (w["b_cf2"], w["b_f2"])
             for j, (r0, rc) in enumerate(ranges):
+                if fp8 and j == 1 and rc > 0:                              # video range in fp8
+                    lnmod8(offs[j] + 0 * d, offs[j] + 1 * d, r0, rc)
+                    qkv8(w["w_qkv"], w["s_qkv"], bq[j], nq[j], nk[j], r0, rc)
+                    continue
                 lnmod(offs[j] + 0 * d, offs[j] + 1 * d, r0, rc)            # (shift_msa, scale_msa) N:173/191
                 qkv(wq[j], bq[j], nq[j], nk[j], r0, rc)
             attention()
             for j, (r0, rc) in enumerate(ranges):
                 if rc == 0:
+                    continue
+                if fp8 and j == 1:
+                    rows = dict(batches=b, rows_per_batch=sl, row_begin=r0, row_count=rc)
+                    quant8(0, wa, r0, rc)
+                    with T("gemm_attn_out"):
+                        ops.gemm_fp8(xn8[:, :, :wa], sc8, w["w_o"], w["s_o"], bo[j], PF_EPI_GATE_RESID, out=h, ldo=d,
+                                     gate=mod[:, offs[j] + 2 * d:], gate_batch_stride=nm, **rows)
+                    lnmod8(offs[j] + 3 * d, offs[j] + 4 * d, r0, rc)
+                    with T("gemm_ff1_gelu"):
+                        ops.gemm_fp8(xa8, sx8, w["w_f1"], w["s_f1"], bf1[j], PF_EPI_GELU_BF16, out=cat, ldo=ldc,
+                                     out_col_begin=wa, **rows)
+                    quant8(wa, ldc, r0, rc)
+                    with T("gemm_ff2"):
+                        ops.gemm_fp8(xn8[:, :, wa:], sc8, w["w_f2"], w["s_f2"], bf2[j], PF_EPI_GATE_RESID, out=h, ldo=d,
+                                     gate=mod[:, offs[j] + 5 * d:], gate_batch_stride=nm, **rows)
                     continue
                 with T("gemm_attn_out"):
                     ops.gemm(cat[:, :, :wa], wo[j], bo[j], PF_EPI_GATE_RESID, batches=b, rows_per_batch=sl, row_begin=r0,
@@ -634,11 +709,24 @@ class B200FluxTransformer(torch.nn.Module):
         n_last = plan.last_tokens
         for i, w in enumerate(self.sgl):
             o = self.mod_off[f"single_transformer_blocks.{i}.norm"]
-            lnmod(o, o + d, 0, sl)                                                                 # (shift, scale) N:232
             # Last block: only the current clip's tokens are read afterwards (F:380), so its queries, MLP and projection
             # run on the rows from the 128-aligned start of the current clip; K/V still cover every token.  Same kernels
             # on fewer rows: the kept rows are bit-identical.  (Single-GPU layout; SP chunks stay uniform.)
             r0 = ((s - n_last) // 128) * 128 if (self.trim_last_block and not par and i == len(self.sgl) - 1) else 0
+            if fp8:
+                rows = dict(batches=b, rows_per_batch=sl, row_begin=r0, row_count=sl - r0)
+                lnmod8(o, o + d, 0, sl)
+                qkv8(w["w_qkv"], w["s_qkv"], w["b_qkv"], w["nq"], w["nk"], 0, sl)
+                with T("gemm_single_mlp_gelu"):
+                    ops.gemm_fp8(xa8, sx8, w["w_mlp"], w["s_mlp"], w["b_mlp"], PF_EPI_GELU_BF16, out=cat, ldo=ldc,
+                                 out_col_begin=wa, **rows)
+                attention(q_row_begin=r0)
+                quant8(0, ldc, r0, sl - r0)
+                with T("gemm_single_out"):
+                    ops.gemm_fp8(xn8, sc8, w["w_out"], w["s_out"], w["b_out"], PF_EPI_GATE_RESID, out=h, ldo=d,
+                                 gate=mod[:, o + 2 * d:], gate_batch_stride=nm, **rows)
+                continue
+            lnmod(o, o + d, 0, sl)                                                                 # (shift, scale) N:232
             # two launches sharing A: measured faster than the fused q|k|v|mlp GEMM (PF_EPI_QKV_GELU), whose 192-wide
             # tiles slow the MLP half down (1.81 ms fused vs 0.60 + 0.62 ms split at S=15488)
             qkv(w["w_qkv"], w["b_qkv"], w["nq"], w["nk"], 0, sl)

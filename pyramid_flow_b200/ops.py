@@ -18,16 +18,16 @@ def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
 
 
-def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], epilogue: int, *,
-         batches: int = 1, rows_per_batch: Optional[int] = None, row_begin: int = 0, row_count: Optional[int] = None,
-         out: Optional[torch.Tensor] = None, ldo: Optional[int] = None, out_batch_rows: Optional[int] = None,
-         out_row_begin: Optional[int] = None, out_col_begin: int = 0,
-         gate: Optional[torch.Tensor] = None, gate_batch_stride: int = 0,
-         q_out=None, k_out=None, v_out=None, rope=None, q_norm_w=None, k_norm_w=None, norm_eps: float = 1e-6,
-         heads: int = 0, head_dim: int = 0, seq_len: int = 0, n_split: int = 0, kernel_variant: int = 0,
-         peer: Optional[dict] = None) -> None:
-    """epilogue(A . W^T + bias); see pf_gemm_bf16 in include/pf_b200.h for the addressing rules."""
-    assert a.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and a.is_cuda and w.is_cuda
+def _gemm_desc(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], epilogue: int, *,
+               batches: int = 1, rows_per_batch: Optional[int] = None, row_begin: int = 0, row_count: Optional[int] = None,
+               out: Optional[torch.Tensor] = None, ldo: Optional[int] = None, out_batch_rows: Optional[int] = None,
+               out_row_begin: Optional[int] = None, out_col_begin: int = 0,
+               gate: Optional[torch.Tensor] = None, gate_batch_stride: int = 0,
+               q_out=None, k_out=None, v_out=None, rope=None, q_norm_w=None, k_norm_w=None, norm_eps: float = 1e-6,
+               heads: int = 0, head_dim: int = 0, seq_len: int = 0, n_split: int = 0, kernel_variant: int = 0,
+               peer: Optional[dict] = None) -> GemmDesc:
+    """The pf_gemm_desc of one launch (operand dtypes are checked by the callers)."""
+    assert a.is_cuda and w.is_cuda
     assert a.stride(-1) == 1 and w.is_contiguous()
     n, k = w.shape
     lda = a.stride(-2)
@@ -65,7 +65,43 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], epilogu
             d.peer_qkv[i] = pp
         d.peer_count, d.peer_heads = len(peer["peer_ptrs"]), peer["peer_heads"]
         d.peer_seq, d.peer_row0 = peer["peer_seq"], peer["peer_row0"]
+    return d
+
+
+def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], epilogue: int, **kw) -> None:
+    """epilogue(A . W^T + bias); see pf_gemm_bf16 in include/pf_b200.h for the addressing rules and `_gemm_desc` for the
+    keyword arguments."""
+    assert a.dtype == torch.bfloat16 and w.dtype == torch.bfloat16
+    d = _gemm_desc(a, w, bias, epilogue, **kw)
     _lib.check(_lib.load().pf_gemm_bf16(C.byref(d), _lib.stream_ptr()), "pf_gemm_bf16")
+
+
+def gemm_fp8(a8: torch.Tensor, a_scale: torch.Tensor, w8: torch.Tensor, w_scale: torch.Tensor, bias: Optional[torch.Tensor],
+             epilogue: int, **kw) -> None:
+    """epilogue((A8 . W8^T) * a_scale[row] * w_scale[n] + bias) on e4m3 operands (pf_gemm_fp8); the keyword arguments are
+    those of `gemm`.  a_scale: fp32 [batches, rows_per_batch] indexed like A's rows; w_scale: fp32 [n]."""
+    assert a8.dtype == torch.float8_e4m3fn and w8.dtype == torch.float8_e4m3fn
+    assert a_scale.dtype == torch.float32 and a_scale.is_contiguous() and w_scale.dtype == torch.float32
+    assert w_scale.is_contiguous() and w_scale.numel() == w8.shape[0]
+    d = _gemm_desc(a8, w8, bias, epilogue, **kw)
+    assert a_scale.numel() >= d.batches * d.rows_per_batch
+    _lib.check(_lib.load().pf_gemm_fp8(C.byref(d), a_scale.data_ptr(), w_scale.data_ptr(), _lib.stream_ptr()), "pf_gemm_fp8")
+
+
+E4M3_MAX = 448.0
+
+
+def quantize_weight_fp8(w: torch.Tensor):
+    """Host quantiser of a weight [N, K] with one scale per output channel (include/pf_b200.h FP8 contract), from the values
+    taken to fp32: -> (w8 float8_e4m3fn [N, K], scale fp32 [N]).  torch's cast does not saturate, but the scaled values stay
+    within 448 (1 + 2^-23), which rounds to 448, so the bits are those of the device quantiser."""
+    w = w.detach().float()
+    amax = w.abs().amax(dim=1)
+    # tensor / tensor divisions are IEEE; with a Python scalar torch may multiply by a reciprocal (two roundings)
+    e4m3_max = torch.full_like(amax, E4M3_MAX)
+    inv = torch.where(amax > 0, e4m3_max / amax, torch.zeros_like(amax))
+    w8 = (w * inv[:, None]).to(torch.float8_e4m3fn).contiguous()
+    return w8, (amax / e4m3_max).contiguous()
 
 
 def linear_bf16(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, gelu: bool = False) -> torch.Tensor:
@@ -83,6 +119,37 @@ def ln_modulate(x: torch.Tensor, y: torch.Tensor, shift: torch.Tensor, scale: to
     _lib.check(_lib.load().pf_ln_modulate(x.data_ptr(), y.data_ptr(), batches, rows_per_batch, row_begin, row_count,
                                           dim, shift.data_ptr(), scale.data_ptr(), mod_batch_stride, eps,
                                           _lib.stream_ptr()), "pf_ln_modulate")
+
+
+def ln_modulate_fp8(x: torch.Tensor, y8: torch.Tensor, row_scale: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor,
+                    mod_batch_stride: int, *, batches: int, rows_per_batch: int, row_begin: int, row_count: int,
+                    eps: float = 1e-6) -> None:
+    """ln_modulate with an e4m3 output y8 [.., dim] (row stride dim) and its per-row scales row_scale fp32
+    [batches, rows_per_batch] (pf_ln_modulate_fp8)."""
+    assert x.dtype == torch.float32 and x.is_contiguous() and y8.dtype == torch.float8_e4m3fn and y8.is_contiguous()
+    assert row_scale.dtype == torch.float32 and row_scale.is_contiguous() and row_scale.numel() >= batches * rows_per_batch
+    dim = x.shape[-1]
+    assert y8.numel() >= batches * rows_per_batch * dim
+    _lib.check(_lib.load().pf_ln_modulate_fp8(x.data_ptr(), y8.data_ptr(), row_scale.data_ptr(), batches, rows_per_batch,
+                                              row_begin, row_count, dim, shift.data_ptr(), scale.data_ptr(),
+                                              mod_batch_stride, eps, _lib.stream_ptr()), "pf_ln_modulate_fp8")
+
+
+def quantize_rows_fp8(x: torch.Tensor, y8: torch.Tensor, row_scale: torch.Tensor, *, batches: int = 1,
+                      rows_per_batch: Optional[int] = None, row_begin: int = 0, row_count: Optional[int] = None) -> None:
+    """x bf16 [(batches,) rows, cols] (row stride x.stride(-2)) -> e4m3 y8 (same shape, row stride y8.stride(-2)) and
+    row_scale fp32 [batches, rows_per_batch], for rows [row_begin, row_begin + row_count) of each batch (pf_quantize_rows_fp8)."""
+    assert x.dtype == torch.bfloat16 and y8.dtype == torch.float8_e4m3fn and x.is_cuda and y8.is_cuda
+    assert x.stride(-1) == 1 and y8.stride(-1) == 1 and x.shape[-1] == y8.shape[-1]
+    assert row_scale.dtype == torch.float32 and row_scale.is_contiguous()
+    if rows_per_batch is None:
+        rows_per_batch = x.shape[-2]
+    if row_count is None:
+        row_count = rows_per_batch - row_begin
+    assert row_scale.numel() >= batches * rows_per_batch
+    _lib.check(_lib.load().pf_quantize_rows_fp8(x.data_ptr(), x.stride(-2), y8.data_ptr(), y8.stride(-2), row_scale.data_ptr(),
+                                                batches, rows_per_batch, row_begin, row_count, x.shape[-1],
+                                                _lib.stream_ptr()), "pf_quantize_rows_fp8")
 
 
 def small_linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], y: torch.Tensor, *, act_in: int = 0,

@@ -1,7 +1,8 @@
 """Time every GEMM family of one DiT step at the step's exact shapes and epilogues (B=2, S=15488 = 128 text + 15360 video
-tokens, 30 heads x 64, FF 4x), through pf_gemm_bf16.
+tokens, 30 heads x 64, FF 4x), through pf_gemm_bf16, or with --fp8 through pf_gemm_fp8 on e4m3 operands (the same rows; the
+rate is printed next to the H100 SXM data-sheet bound, 989 TFLOP/s dense bf16 and 1,979 dense fp8, a bound that is not reached).
 
-    python tools/gemm_bench.py [--iters 30] [--warmup 5] [--json out.json]
+    python tools/gemm_bench.py [--fp8] [--iters 30] [--warmup 5] [--json out.json]
 
 Each row is timed with CUDA events around `iters` back-to-back launches after `warmup` launches of the same shape; the rate is
 2*M*N*K over the mean launch time.  Operands are re-read every launch, and every row's working set (A + W + output) is larger
@@ -57,8 +58,10 @@ def main():
     ap.add_argument("--iters", type=int, default=30)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--kernel-variant", type=int, default=0, help="pf_gemm_desc.kernel_variant (0 = automatic choice)")
+    ap.add_argument("--fp8", action="store_true", help="pf_gemm_fp8 on e4m3 operands with per-row / per-channel scales")
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
+    bound = 1979.0 if args.fp8 else 989.0
     _lib.require_device()
     dev = "cuda"
     g = torch.Generator(device=dev).manual_seed(0)
@@ -71,6 +74,10 @@ def main():
     nq = 1 + 0.1 * torch.randn(HD, device=dev, generator=g)
     nk = 1 + 0.1 * torch.randn(HD, device=dev, generator=g)
     gate = torch.randn(B, D, device=dev, generator=g) * 0.01
+    if args.fp8:
+        xn8 = torch.empty(B, S, 5 * D, device=dev, dtype=torch.float8_e4m3fn)
+        sa = torch.empty(B, S, device=dev)
+        ops.quantize_rows_fp8(xn, xn8, sa, batches=B, rows_per_batch=S)
     info = card()
     print(f"[gemm_bench] {info['name']} | nvidia-smi name, power limit, max SM clock: {info['nvidia_smi']}")
     print(f"[gemm_bench] CUDA events over {args.iters} back-to-back launches after {args.warmup} warm-up launches; "
@@ -79,6 +86,9 @@ def main():
     for name, r0, rc, n, kk, epi, per_step in ROWS:
         a = xn[:, :, :kk]
         w = (torch.randn(n, kk, device=dev, generator=g) * 0.02).bfloat16()
+        if args.fp8:
+            w8, sw = (t.to(dev) for t in ops.quantize_weight_fp8(w.cpu()))
+            a8 = xn8[:, :, :kk]
         bias = torch.randn(n, device=dev, generator=g) * 0.1
         if epi == PF_EPI_QKV_ROPE:
             kw = dict(q_out=q, k_out=k, v_out=v, rope=rope, q_norm_w=nq, k_norm_w=nk, heads=H, head_dim=HD, seq_len=S)
@@ -91,8 +101,11 @@ def main():
             out_bytes = 2 * B * rc * n * 4
 
         def launch():
-            ops.gemm(a, w, bias, epi, batches=B, rows_per_batch=S, row_begin=r0, row_count=rc,
-                     kernel_variant=args.kernel_variant, **kw)
+            if args.fp8:
+                ops.gemm_fp8(a8, sa, w8, sw, bias, epi, batches=B, rows_per_batch=S, row_begin=r0, row_count=rc, **kw)
+            else:
+                ops.gemm(a, w, bias, epi, batches=B, rows_per_batch=S, row_begin=r0, row_count=rc,
+                         kernel_variant=args.kernel_variant, **kw)
         for _ in range(args.warmup):
             launch()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -104,19 +117,22 @@ def main():
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / args.iters
         flop = 2.0 * B * rc * n * kk
-        ws = B * rc * kk * 2 + n * kk * 2 + out_bytes
+        esz = 1 if args.fp8 else 2
+        ws = B * rc * kk * esz + n * kk * esz + out_bytes
         tf = flop / (ms * 1e-3) / 1e12
         total_ms += ms * per_step
         total_flop += flop * per_step
         rows.append(dict(family=name, m=B * rc, n=n, k=kk, ms=round(ms, 4), tflops=round(tf, 1), per_step=per_step,
                          working_set_mb=round(ws / 2**20, 1)))
-        print(f"  {name:24s} M={B * rc:6d} N={n:5d} K={kk:5d}  {ms * 1e3:9.1f} us  {tf:6.1f} TFLOP/s  "
+        print(f"  {name:24s} M={B * rc:6d} N={n:5d} K={kk:5d}  {ms * 1e3:9.1f} us  {tf:6.1f} TFLOP/s "
+              f"(data-sheet bound {bound:.0f})  "
               f"x{per_step:2d}/step  working set {ws / 2**20:7.1f} MB {'> L2' if ws > L2_BYTES else '< L2'}")
     print(f"[gemm_bench] per-step GEMM total (rows above x launches/step): {total_ms:.2f} ms, "
           f"{total_flop / (total_ms * 1e-3) / 1e12:.1f} TFLOP/s")
     if args.json:
         Path(args.json).parent.mkdir(parents=True, exist_ok=True)
-        Path(args.json).write_text(json.dumps(dict(card=info, rows=rows, step_total_ms=round(total_ms, 3)), indent=1))
+        Path(args.json).write_text(json.dumps(dict(card=info, fp8=args.fp8, rows=rows, step_total_ms=round(total_ms, 3)),
+                                              indent=1))
 
 
 if __name__ == "__main__":
