@@ -43,6 +43,7 @@ import torch.nn.functional as F
 
 from . import _lib, ops
 from ._lib import PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_ROPE, PF_EPI_STORE_F32
+from .graphs import GraphedStep
 
 
 @dataclass
@@ -142,6 +143,18 @@ class _Cfg(dict):
     __getattr__ = dict.__getitem__
 
 
+def check_gemm_precision(gemm_precision: str) -> None:
+    if gemm_precision not in ("bf16", "fp8"):
+        raise ValueError(f"gemm_precision must be 'bf16' or 'fp8', not {gemm_precision!r}")
+
+
+def fp8_weight(sd: Dict[str, torch.Tensor], names: Sequence[str], device):
+    """The state-dict weights `names` concatenated along the output dim, quantised once on the host from their fp32 values:
+    (e4m3 [N, K], fp32 per-output-channel scale [N]) on `device`; no bf16 copy is kept."""
+    w8, sc = ops.quantize_weight_fp8(torch.cat([sd[n + ".weight"].float().cpu() for n in names], 0))
+    return w8.to(device), sc.to(device)
+
+
 class _KernelTimer:
     """Optional CUDA-event timing of kernel families inside a step (bench.py breakdown); disabled => zero overhead."""
 
@@ -184,14 +197,13 @@ class _NullSpan:
 _NULL_SPAN = _NullSpan()
 
 
-class B200FluxTransformer(torch.nn.Module):
+class B200FluxTransformer(GraphedStep, torch.nn.Module):
     """Holder of packed bf16 weights + the kernel-launch sequence of one DiT step."""
 
     def __init__(self, config: FluxConfigB200, state_dict: Dict[str, torch.Tensor], device="cuda",
                  emulate_bf16_rounding: bool = False, gemm_precision: str = "bf16"):
         super().__init__()
-        if gemm_precision not in ("bf16", "fp8"):
-            raise ValueError(f"gemm_precision must be 'bf16' or 'fp8', not {gemm_precision!r}")
+        check_gemm_precision(gemm_precision)
         # "fp8": the block GEMMs listed in the module docstring run on e4m3 operands (opt-in: different numerics)
         self.gemm_precision = gemm_precision
         self.cfg = config
@@ -211,18 +223,9 @@ class B200FluxTransformer(torch.nn.Module):
         self._last_key = None
         self.attn_events = None   # bench.py: list collecting (start, end) CUDA events around every attention launch
         self.timer = _KernelTimer()
-        # CUDA graphs: the ~290 launches of a step are captured once per (plan, input shapes) and replayed, so the step
-        # does not depend on how fast the host can walk the launch sequence (ctypes + descriptor encoding per launch).
-        # Off by default: callers that reuse shapes for many steps (sampler, bench) turn it on.
         self.trim_last_block = True     # last single block on the current clip's rows only (exact; see forward)
         self.attn_variant = 0           # pf_attn_desc.variant (every value runs the one sm_90a kernel)
-        self.use_cuda_graph = False
-        self._graphs: "Dict[tuple, dict]" = {}
-        self._graph_warm = False
-        self._graph_pool = None
-        self._graph_stream = None
-        self.graph_replays = 0          # bookkeeping for bench.py: replays and kernel launches replayed
-        self.graph_launches_replayed = 0
+        self._init_graphs()             # use_cuda_graph: the ~290 launches of a step captured once per shape (graphs.py)
 
     @classmethod
     def from_reference(cls, ref_module, device="cuda", **kw) -> "B200FluxTransformer":
@@ -252,9 +255,8 @@ class B200FluxTransformer(torch.nn.Module):
         fp8 = self.gemm_precision == "fp8"
 
         def WQ(blk, key, *names):   # the weight of a GEMM that runs in fp8 under gemm_precision="fp8"
-            if fp8:                 # e4m3 [N, K] + fp32 per-channel scale "s_..." from the fp32 values (host), no bf16 copy
-                w8, sc = ops.quantize_weight_fp8(torch.cat([sd[n + ".weight"].float().cpu() for n in names], 0))
-                blk[key], blk["s" + key[1:]] = w8.to(device), sc.to(device)
+            if fp8:
+                blk[key], blk["s" + key[1:]] = fp8_weight(sd, names, device)
             else:
                 blk[key] = W(*names)
 
@@ -444,71 +446,21 @@ class B200FluxTransformer(torch.nn.Module):
         return self._forward_eager(clips, timestep_ratio, encoder_hidden_states, encoder_attention_mask,
                                    pooled_projections)
 
-    def _forward_graphed(self, clips, timestep_ratio, enc, mask, pooled):
-        """Replay the step's captured launch sequence; inputs are copied into the capture's static buffers."""
-        dev = self.device
-        plan = self.plan_for([cl.shape for cl in clips], mask)
-        ins = [*clips, timestep_ratio, enc, pooled]
-        key = (id(plan), bool(getattr(self, "output_fp32", False)), bool(self.trim_last_block),
-               bool(self.emulate_bf16_rounding), int(self.attn_variant), tuple((tuple(x.shape), x.dtype) for x in ins))
-        ent = self._graphs.get(key)
-        if ent is None:
-            while len(self._graphs) >= 3:                      # every entry pins a workspace (~1.5 GB at 768p)
-                self._graphs.pop(next(iter(self._graphs)))
-            static = [torch.empty(x.shape, dtype=x.dtype, device=dev) for x in ins]
-            for st, x in zip(static, ins):
-                st.copy_(x, non_blocking=True)
-            nclip = len(clips)
+    # -- CUDA-graph replay (graphs.GraphedStep) -------------------------------------------------------------------------
+    def _graph_key_fields(self) -> tuple:
+        return (bool(getattr(self, "output_fp32", False)), bool(self.trim_last_block), bool(self.emulate_bf16_rounding),
+                int(self.attn_variant))
 
-            def run():
-                return self._forward_eager(static[:nclip], static[nclip], static[nclip + 1], mask, static[nclip + 2])[0]
-
-            # allocate outside the capture (ordinary allocator pool); the parallel layout also (re)builds its peer arena here,
-            # a collective that must not happen inside stream capture
-            lay = getattr(self, "layout", None)
-            if lay is not None and lay.enabled:
-                from . import sp as SP
-                c0, c1 = SP.chunk_bounds(plan.seq, lay.sp, lay.sp_rank)
-                self._workspace(1, plan, c1 - c0, self._hp)
-                if getattr(self, "exchange", DEFAULT_EXCHANGE) == "peer":
-                    self._peer_exchange(plan, self._hp, self._hp * 64 + 4 * self.cfg.inner_dim)
-            else:
-                self._workspace(clips[-1].shape[0], plan)
-            # Nothing host-side may initialise inside stream capture: `_lib.require_device()` has already loaded every kernel
-            # instantiation and set its shared-memory attribute on this device (pf_warmup), so a new shape that
-            # dispatches to a not-yet-used template instantiation is safe to capture; the first capture of the process
-            # additionally runs the step once host-launched (allocator pools, plan upload).
-            if not self._graph_warm:
-                run()
-                self._graph_warm = True
-            # Manual capture on a side stream (what torch.cuda.graph() does, minus its gc.collect() + empty_cache(), which
-            # cost ~50 ms per capture and made the per-(unit, stage) captures of the sampler a net loss at 384p); all
-            # graphs share one memory pool, so the buffers of an evicted graph are reused by the next capture.
-            if self._graph_pool is None:
-                self._graph_pool = torch.cuda.graph_pool_handle()
-                self._graph_stream = torch.cuda.Stream()
-            graph = torch.cuda.CUDAGraph()
-            n0 = _lib.launch_count()
-            side = self._graph_stream
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                graph.capture_begin(pool=self._graph_pool)
-                try:
-                    out = run()
-                finally:
-                    graph.capture_end()
-            torch.cuda.current_stream().wait_stream(side)
-            ent = dict(graph=graph, static=static, out=out, launches=_lib.launch_count() - n0, plan=plan, mask=mask,
-                       ws=dict(self._ws))   # the captured pointers must stay allocated as long as the graph lives
-            self._graphs[key] = ent
+    def _graph_prealloc(self, plan: SeqPlan, clips) -> None:
+        lay = getattr(self, "layout", None)
+        if lay is not None and lay.enabled:
+            from . import sp as SP
+            c0, c1 = SP.chunk_bounds(plan.seq, lay.sp, lay.sp_rank)
+            self._workspace(1, plan, c1 - c0, self._hp)
+            if getattr(self, "exchange", DEFAULT_EXCHANGE) == "peer":
+                self._peer_exchange(plan, self._hp, self._hp * 64 + 4 * self.cfg.inner_dim)
         else:
-            for st, x in zip(ent["static"], ins):
-                st.copy_(x, non_blocking=True)
-        self.last_plan = ent["plan"]
-        ent["graph"].replay()
-        self.graph_replays += 1
-        self.graph_launches_replayed += ent["launches"]
-        return [ent["out"].clone()]
+            self._workspace(clips[-1].shape[0], plan)
 
     def _forward_eager(self, clips, timestep_ratio=None, encoder_hidden_states=None, encoder_attention_mask=None,
                        pooled_projections=None):

@@ -9,6 +9,15 @@ Reuses the miniFLUX kernels unchanged — 24 double blocks at D=1536 / 24 heads 
   * RoPE table = ONE 64-wide axis over the running frame index (modeling_pyramid_mmdit.py:116, 235-262, 301-305);
   * the last block is `context_pre_only`: AdaLayerNormContinuous (scale, shift) on the text stream, no text update after
     attention (modeling_mmdit_block.py:585-622, 659-660); q/k RMSNorm eps is 1e-5 (JointAttention default, MB:409).
+
+gemm_precision="fp8" (opt-in, changes the numerics; include/pf_b200.h FP8 contract): the video-range QKV, to_out, FF1 and FF2
+GEMMs of every joint block, the video stream of the context_pre_only last block included, run on e4m3 operands (per-token
+activation scales, per-output-channel weight scales quantised once at import), as in dit.py.  The text stream (add_*_proj,
+to_add_out, ff_context), the patch embed, the context embedder, the head and the conditioning / AdaLN GEMVs stay bf16.
+The workspace gains dit.py's `xn8` (e4m3 twin of `cat`, its first B*S*D bytes also holding the LN-modulate output), `sx8`
+and `sc8` (row scales).
+
+use_cuda_graph = True captures each (plan, input shapes and dtypes, precision) once and replays it (graphs.GraphedStep).
 """
 from __future__ import annotations
 
@@ -20,7 +29,8 @@ import torch.nn.functional as F
 
 from . import _lib, ops
 from ._lib import PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_ROPE, PF_EPI_STORE_F32
-from .dit import SeqPlan, build_rope_table, _Cfg
+from .dit import SeqPlan, build_rope_table, check_gemm_precision, fp8_weight, _Cfg
+from .graphs import GraphedStep
 from dataclasses import dataclass
 
 
@@ -40,9 +50,13 @@ class MMDiTConfigB200:
         return self.num_attention_heads * self.attention_head_dim
 
 
-class B200MMDiT(torch.nn.Module):
-    def __init__(self, config: MMDiTConfigB200, state_dict: Dict[str, torch.Tensor], device="cuda"):
+class B200MMDiT(GraphedStep, torch.nn.Module):
+    def __init__(self, config: MMDiTConfigB200, state_dict: Dict[str, torch.Tensor], device="cuda",
+                 gemm_precision: str = "bf16"):
         super().__init__()
+        check_gemm_precision(gemm_precision)
+        # "fp8": the block GEMMs listed in the module docstring run on e4m3 operands (opt-in: different numerics)
+        self.gemm_precision = gemm_precision
         self.cfg = config
         self.config = _Cfg(in_channels=config.in_channels, num_layers=config.num_layers,
                            num_attention_heads=config.num_attention_heads, attention_head_dim=config.attention_head_dim,
@@ -52,15 +66,16 @@ class B200MMDiT(torch.nn.Module):
         self._plans, self._ws, self._last_key = {}, {}, None
         self.last_plan: Optional[SeqPlan] = None
         self._import_state_dict(state_dict, torch.device(device))
+        self._init_graphs()
 
     @classmethod
-    def from_reference(cls, ref_module, device="cuda") -> "B200MMDiT":
+    def from_reference(cls, ref_module, device="cuda", **kw) -> "B200MMDiT":
         rc = ref_module.config
         cfg = MMDiTConfigB200(num_layers=rc.num_layers, num_attention_heads=rc.num_attention_heads,
                               attention_head_dim=rc.attention_head_dim, in_channels=rc.in_channels,
                               patch_size=rc.patch_size, joint_attention_dim=rc.joint_attention_dim,
                               pooled_projection_dim=rc.pooled_projection_dim, pos_embed_max_size=rc.pos_embed_max_size)
-        return cls(cfg, ref_module.state_dict(), device=device)
+        return cls(cfg, ref_module.state_dict(), device=device, **kw)
 
     def _import_state_dict(self, sd, device) -> None:
         c = self.cfg
@@ -74,6 +89,14 @@ class B200MMDiT(torch.nn.Module):
 
         def V(name):
             return sd[name].float().to(device).contiguous()
+
+        fp8 = self.gemm_precision == "fp8"
+
+        def WQ(blk, key, *names):   # the weight of a GEMM that runs in fp8 under gemm_precision="fp8"
+            if fp8:
+                blk[key], blk["s" + key[1:]] = fp8_weight(sd, names, device)
+            else:
+                blk[key] = W(*names)
 
         reg = self.register_buffer
         for a, n in (("t1", "time_text_embed.timestep_embedder.linear_1"), ("t2", "time_text_embed.timestep_embedder.linear_2"),
@@ -100,16 +123,17 @@ class B200MMDiT(torch.nn.Module):
             p = f"transformer_blocks.{i}"
             last = i == c.num_layers - 1
             blk = dict(
-                w_qkv=W(p + ".attn.to_q", p + ".attn.to_k", p + ".attn.to_v"),
                 b_qkv=Bv(p + ".attn.to_q", p + ".attn.to_k", p + ".attn.to_v"),
                 w_cqkv=W(p + ".attn.add_q_proj", p + ".attn.add_k_proj", p + ".attn.add_v_proj"),
                 b_cqkv=Bv(p + ".attn.add_q_proj", p + ".attn.add_k_proj", p + ".attn.add_v_proj"),
                 nq=V(p + ".attn.norm_q.weight"), nk=V(p + ".attn.norm_k.weight"),
                 cnq=V(p + ".attn.norm_add_q.weight"), cnk=V(p + ".attn.norm_add_k.weight"),
-                w_o=W(p + ".attn.to_out.0"), b_o=Bv(p + ".attn.to_out.0"),
-                w_f1=W(p + ".ff.net.0.proj"), b_f1=Bv(p + ".ff.net.0.proj"),
-                w_f2=W(p + ".ff.net.2"), b_f2=Bv(p + ".ff.net.2"),
+                b_o=Bv(p + ".attn.to_out.0"), b_f1=Bv(p + ".ff.net.0.proj"), b_f2=Bv(p + ".ff.net.2"),
             )
+            WQ(blk, "w_qkv", p + ".attn.to_q", p + ".attn.to_k", p + ".attn.to_v")
+            WQ(blk, "w_o", p + ".attn.to_out.0")
+            WQ(blk, "w_f1", p + ".ff.net.0.proj")
+            WQ(blk, "w_f2", p + ".ff.net.2")
             if not last:
                 blk.update(w_co=W(p + ".attn.to_add_out"), b_co=Bv(p + ".attn.to_add_out"),
                            w_cf1=W(p + ".ff_context.net.0.proj"), b_cf1=Bv(p + ".ff_context.net.0.proj"),
@@ -195,6 +219,10 @@ class B200MMDiT(torch.nn.Module):
                       temb=torch.empty(b, d, device=dev, dtype=torch.float32),
                       tmp=torch.empty(b, d, device=dev, dtype=torch.float32),
                       head=torch.empty(b, plan.last_tokens, 4 * c.in_channels, device=dev, dtype=torch.float32))
+            if self.gemm_precision == "fp8":
+                ws["xn8"] = torch.empty(b, sl, 5 * d, device=dev, dtype=torch.float8_e4m3fn)
+                ws["sx8"] = torch.empty(b, sl, device=dev, dtype=torch.float32)
+                ws["sc8"] = torch.empty(b, sl, device=dev, dtype=torch.float32)
             self._ws[key] = ws
         return ws
 
@@ -204,12 +232,24 @@ class B200MMDiT(torch.nn.Module):
         the attention output cross NVLink as remote stores fused into the QKV-GEMM / attention epilogues (csrc/pf_peer.cu), as
         in B200FluxTransformer.  The reference runs this model with sp 2 or 4 (scripts/inference_multigpu.sh:9); 24 heads
         divide by both, so no head padding is needed."""
+        if self.gemm_precision == "fp8":
+            raise NotImplementedError("gemm_precision='fp8' runs on one GPU only: the sequence-parallel peer-store epilogues "
+                                      "have no fp8 form (build the model with gemm_precision='bf16' for a parallel layout)")
         assert self.cfg.num_attention_heads % max(1, layout.sp) == 0, "heads must divide by the SP degree"
         if layout.sp > 1:   # see _lib.load(): one attention kernel for the whole process once sequence parallelism is in play
             _lib.set_option(_lib.PF_OPT_ATTN_TRIPLE_KERNEL, 0)
         self.layout = layout
         self._px = None
+        self._graphs.clear()
         self._ws.clear()
+
+    def _peer_exchange(self, plan: SeqPlan):
+        """The peer arena (sp.PeerExchange) for this call's shapes; see sp.ensure_peer_exchange."""
+        from . import sp as SP
+        c = self.cfg
+        ct, chh, cww = plan.clip_thw[-1]
+        return SP.ensure_peer_exchange(self, self.layout, plan.seq, plan.last_tokens, c.num_attention_heads, 5 * c.inner_dim,
+                                       4 * c.in_channels, c.in_channels * ct * chh * 2 * cww * 2 * 4)
 
     @torch.no_grad()
     def forward(self, sample, timestep_ratio=None, encoder_hidden_states=None, encoder_attention_mask=None,
@@ -217,6 +257,30 @@ class B200MMDiT(torch.nn.Module):
         _lib.require_device()
         assert len(sample) == 1
         clips = sample[0] if isinstance(sample[0], (list, tuple)) else [sample[0]]
+        if self.use_cuda_graph:
+            return self._forward_graphed(list(clips), timestep_ratio, encoder_hidden_states, encoder_attention_mask,
+                                         pooled_projections)
+        return self._forward_eager(clips, timestep_ratio, encoder_hidden_states, encoder_attention_mask, pooled_projections)
+
+    # -- CUDA-graph replay (graphs.GraphedStep) -------------------------------------------------------------------------
+    def _graph_plan(self, clips, mask):   # (plan, positional table): the captured device copy into `h` reads the table
+        return self.plan_for([cl.shape for cl in clips], mask)
+
+    def _graph_key_fields(self) -> tuple:
+        return (self.gemm_precision,)
+
+    def _graph_prealloc(self, plan: SeqPlan, clips) -> None:
+        lay = getattr(self, "layout", None)
+        if lay is not None and lay.enabled:
+            from . import sp as SP
+            c0, c1 = SP.chunk_bounds(plan.seq, lay.sp, lay.sp_rank)
+            self._workspace(1, plan, c1 - c0)
+            self._peer_exchange(plan)
+        else:
+            self._workspace(clips[-1].shape[0], plan)
+
+    def _forward_eager(self, clips, timestep_ratio=None, encoder_hidden_states=None, encoder_attention_mask=None,
+                       pooled_projections=None):
         c = self.cfg
         d, hn = c.inner_dim, c.num_attention_heads
         bg = clips[-1].shape[0]
@@ -239,9 +303,7 @@ class B200MMDiT(torch.nn.Module):
         ldc = 5 * d
         px = None
         if par:
-            ct_, ch_, cw_ = plan.clip_thw[-1]
-            px = SP.ensure_peer_exchange(self, lay, s, plan.last_tokens, hn, ldc, 4 * c.in_channels,
-                                         c.in_channels * ct_ * ch_ * 2 * cw_ * 2 * 4)
+            px = self._peer_exchange(plan)
             if nsp > 1:
                 cat = px.cat(sl)
                 qkv_x = px.qkv(s)
@@ -282,6 +344,19 @@ class B200MMDiT(torch.nn.Module):
                 ops.ln_modulate(h, xn, mod[:, off_shift:], mod[:, off_scale:], nm, batches=b, rows_per_batch=sl, row_begin=r0,
                                 row_count=rc)
 
+        fp8 = self.gemm_precision == "fp8"       # single GPU only (set_parallel_layout), so the video rows are ranges[1]
+        if fp8:
+            xn8, sx8, sc8 = ws["xn8"], ws["sx8"], ws["sc8"]
+            xa8 = xn8.view(-1)[:b * sl * d].view(b, sl, d)    # LN-modulate output, row stride d (module docstring)
+
+        def lnmod8(off_shift, off_scale, r0, rc):
+            ops.ln_modulate_fp8(h, xa8, sx8, mod[:, off_shift:], mod[:, off_scale:], nm, batches=b, rows_per_batch=sl,
+                                row_begin=r0, row_count=rc)
+
+        def quant8(col0, col1, r0, rc):   # cat[:, r0:r0 + rc, col0:col1] -> the same block of xn8, row scales -> sc8
+            ops.quantize_rows_fp8(cat[:, :, col0:col1], xn8[:, :, col0:col1], sc8, batches=b, rows_per_batch=sl, row_begin=r0,
+                                  row_count=rc)
+
         peer_qkv = None
         if px is not None and nsp > 1:
             peer_qkv = dict(peer_ptrs=[pp + px.off_qkv for pp in px.sp_buf.ptrs], peer_heads=hn // nsp, peer_seq=s, peer_row0=c0)
@@ -297,9 +372,16 @@ class B200MMDiT(torch.nn.Module):
                 lnmod(oc + d, oc, *ranges[0])
             else:
                 lnmod(oc, oc + d, *ranges[0])
-            lnmod(ov, ov + d, *ranges[1])
+            if fp8 and ranges[1][1] > 0:
+                lnmod8(ov, ov + d, *ranges[1])
+            else:
+                lnmod(ov, ov + d, *ranges[1])
             for j, (r0, rc) in enumerate(ranges):
-                if rc > 0:
+                if fp8 and j == 1 and rc > 0:
+                    ops.gemm_fp8(xa8, sx8, w["w_qkv"], w["s_qkv"], w["b_qkv"], PF_EPI_QKV_ROPE, batches=b, rows_per_batch=sl,
+                                 row_begin=r0, row_count=rc, q_out=q, k_out=k, v_out=v, rope=rope, q_norm_w=w["nq"],
+                                 k_norm_w=w["nk"], norm_eps=1e-5, heads=hn, head_dim=64, seq_len=sl)
+                elif rc > 0:
                     ops.gemm(xn, (w["w_cqkv"], w["w_qkv"])[j], (w["b_cqkv"], w["b_qkv"])[j], PF_EPI_QKV_ROPE, batches=b,
                              rows_per_batch=sl, row_begin=r0, row_count=rc, q_out=q, k_out=k, v_out=v, rope=rope,
                              q_norm_w=(w["cnq"], w["nq"])[j], k_norm_w=(w["cnk"], w["nk"])[j], norm_eps=1e-5, heads=hn,
@@ -315,6 +397,18 @@ class B200MMDiT(torch.nn.Module):
             for j, (r0, rc) in enumerate(ranges):
                 if rc == 0 or (j == 0 and last):
                     continue   # context_pre_only: the text stream ends here (MB:659-660)
+                if fp8 and j == 1:
+                    rows = dict(batches=b, rows_per_batch=sl, row_begin=r0, row_count=rc)
+                    quant8(0, d, r0, rc)
+                    ops.gemm_fp8(xn8[:, :, :d], sc8, w["w_o"], w["s_o"], w["b_o"], PF_EPI_GATE_RESID, out=h, ldo=d,
+                                 gate=mod[:, offs[j] + 2 * d:], gate_batch_stride=nm, **rows)
+                    lnmod8(offs[j] + 3 * d, offs[j] + 4 * d, r0, rc)
+                    ops.gemm_fp8(xa8, sx8, w["w_f1"], w["s_f1"], w["b_f1"], PF_EPI_GELU_BF16, out=cat, ldo=ldc, out_col_begin=d,
+                                 **rows)
+                    quant8(d, ldc, r0, rc)
+                    ops.gemm_fp8(xn8[:, :, d:], sc8, w["w_f2"], w["s_f2"], w["b_f2"], PF_EPI_GATE_RESID, out=h, ldo=d,
+                                 gate=mod[:, offs[j] + 5 * d:], gate_batch_stride=nm, **rows)
+                    continue
                 wo, bo = ((w.get("w_co"), w["w_o"])[j], (w.get("b_co"), w["b_o"])[j])
                 wf1, bf1 = ((w.get("w_cf1"), w["w_f1"])[j], (w.get("b_cf1"), w["b_f1"])[j])
                 wf2, bf2 = ((w.get("w_cf2"), w["w_f2"])[j], (w.get("b_cf2"), w["b_f2"])[j])

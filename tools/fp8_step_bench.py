@@ -1,12 +1,15 @@
-"""The DiT step (bench.py's workload: B=2, S=15488, 8 double + 16 single blocks, synthetic weights) with bf16 GEMMs and with
-gemm_precision="fp8", built from the same weights and timed in one process.
+"""The DiT step with bf16 GEMMs and with gemm_precision="fp8", built from the same synthetic weights and timed in one process.
 
-    python tools/fp8_step_bench.py [--steps 10] [--warmup 3] [--rounds 3] [--json out.json]
+    python tools/fp8_step_bench.py [--model flux|mmdit] [--steps 10] [--warmup 3] [--rounds 3] [--json out.json]
+
+--model flux (default): bench.py's miniFLUX workload (B=2, S=15488, 8 double + 16 single blocks).
+--model mmdit: bench.py --model mmdit's SD3 MMDiT workload (B=2, S=11888, 24 joint blocks, D=1536).
 
 Each round times `steps` graph-replayed steps of the bf16 model, then of the fp8 model (CUDA events, after `warmup` steps),
-so that the two alternate `rounds` times.  Then one extra step per precision runs host-launched with the model's kernel-family
-timer (CUDA events around every launch: the quantise passes are "quantize_fp8"), and the velocity of each precision is
-compared with the other's.  The card's name, power limit and max SM clock are read with nvidia-smi (a query only).
+so that the two alternate `rounds` times.  Then one extra step per precision runs host-launched, and the velocity of each
+precision is compared with the other's (fp32 stores).  For miniFLUX that step also runs the model's kernel-family timer
+(CUDA events around every launch: the quantise passes are "quantize_fp8").  The card's name, power limit and max SM clock
+are read with nvidia-smi (a query only).
 """
 import argparse
 import json
@@ -20,9 +23,10 @@ sys.path.insert(0, str(ROOT))
 
 import torch  # noqa: E402
 
-from bench import random_flux_state_dict, step_clip_shapes  # noqa: E402
+from bench import random_flux_state_dict, random_mmdit_state_dict, step_clip_shapes  # noqa: E402
 from pyramid_flow_b200 import _lib  # noqa: E402
 from pyramid_flow_b200.dit import B200FluxTransformer  # noqa: E402
+from pyramid_flow_b200.mmdit import B200MMDiT, MMDiTConfigB200  # noqa: E402
 
 
 def card():
@@ -35,8 +39,36 @@ def card():
     return {"name": torch.cuda.get_device_name(0), "nvidia_smi": out or "unavailable"}
 
 
+def flux_models(dev):
+    cfg, sd = random_flux_state_dict({}, dev, seed=0)
+    models = {p: B200FluxTransformer(cfg, sd, device=dev, gemm_precision=p) for p in ("bf16", "fp8")}
+    g = torch.Generator().manual_seed(100)
+    call = dict(sample=[[torch.randn(s, generator=g).bfloat16().to(dev) for s in step_clip_shapes(2)]],
+                timestep_ratio=torch.tensor([3.0, 3.0]).bfloat16().to(dev),
+                encoder_hidden_states=(torch.randn(2, 128, 4096, generator=g) * 0.2).bfloat16().to(dev),
+                encoder_attention_mask=torch.ones(2, 128, dtype=torch.int64, device=dev),
+                pooled_projections=torch.randn(2, 768, generator=g).bfloat16().to(dev))
+    return models, call
+
+
+def mmdit_models(dev):
+    """bench.run_mmdit's model and inputs: S = 128 + 13x240 + 960 + 2x3840 = 11888."""
+    cfg = MMDiTConfigB200()
+    sd = random_mmdit_state_dict(cfg, dev)
+    models = {p: B200MMDiT(cfg, sd, device=dev, gemm_precision=p) for p in ("bf16", "fp8")}
+    g = torch.Generator().manual_seed(100)
+    shapes = [(2, 16, 13, 24, 40), (2, 16, 1, 48, 80), (2, 16, 1, 96, 160), (2, 16, 1, 96, 160)]
+    call = dict(sample=[[torch.randn(s, generator=g).bfloat16().to(dev) for s in shapes]],
+                encoder_hidden_states=(torch.randn(2, 128, 4096, generator=g) * 0.2).bfloat16().to(dev),
+                encoder_attention_mask=torch.ones(2, 128, dtype=torch.int64, device=dev),
+                pooled_projections=torch.randn(2, 2048, generator=g).bfloat16().to(dev),
+                timestep_ratio=torch.tensor([3.0, 3.0]).bfloat16().to(dev))
+    return models, call
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--model", default="flux", choices=["flux", "mmdit"])
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--rounds", type=int, default=3)
@@ -47,16 +79,8 @@ def main():
     info = card()
     print(f"[fp8_step_bench] {info['name']} | nvidia-smi name, power limit, max SM clock: {info['nvidia_smi']}")
 
-    cfg, sd = random_flux_state_dict({}, dev, seed=0)
-    models = {p: B200FluxTransformer(cfg, sd, device=dev, gemm_precision=p) for p in ("bf16", "fp8")}
-    del sd
+    models, call = (flux_models if args.model == "flux" else mmdit_models)(dev)
     torch.cuda.empty_cache()
-    g = torch.Generator().manual_seed(100)
-    call = dict(sample=[[torch.randn(s, generator=g).bfloat16().to(dev) for s in step_clip_shapes(2)]],
-                timestep_ratio=torch.tensor([3.0, 3.0]).bfloat16().to(dev),
-                encoder_hidden_states=(torch.randn(2, 128, 4096, generator=g) * 0.2).bfloat16().to(dev),
-                encoder_attention_mask=torch.ones(2, 128, dtype=torch.int64, device=dev),
-                pooled_projections=torch.randn(2, 768, generator=g).bfloat16().to(dev))
 
     def timed(model):
         for _ in range(args.warmup):
@@ -84,6 +108,9 @@ def main():
     breakdown, vel = {}, {}
     for p, m in models.items():
         m.use_cuda_graph = False
+        if args.model == "mmdit":   # fp32 clips holding the same bf16 values: the same step with an fp32 velocity store
+            vel[p] = m(**dict(call, sample=[[c.float() for c in call["sample"][0]]]))[0]
+            continue
         m.output_fp32 = True
         m.timer.enabled = True
         m.timer.events = []
@@ -103,8 +130,8 @@ def main():
     print(f"[fp8_step_bench] fp8 velocity vs bf16 velocity (fp32 stores): {err}")
     if args.json:
         Path(args.json).parent.mkdir(parents=True, exist_ok=True)
-        Path(args.json).write_text(json.dumps(dict(card=info, ms_per_step=ms, median_ms=med, breakdown_ms=breakdown,
-                                                   fp8_vs_bf16=err), indent=1))
+        Path(args.json).write_text(json.dumps(dict(card=info, model=args.model, ms_per_step=ms, median_ms=med,
+                                                   breakdown_ms=breakdown, fp8_vs_bf16=err), indent=1))
 
 
 if __name__ == "__main__":
