@@ -4,6 +4,7 @@ Call surface used by the pipeline (pyramid_dit_for_video_gen_pipeline.py:1221-12
 
     self.vae.decode(latents, temporal_chunk=True, window_size=w, tile_sample_min_size=s).sample    # [B, 3, T', H', W']
     self.vae.encode(image[:, :, None]).latent_dist.sample()                                        # i2v image latent
+    self.vae.encode(video, temporal_chunk=True, window_size=16, tile_sample_min_size=256)          # training latents
 
 plus `.device`, `.dtype`, `.to()`, `.enable_tiling()`.  Weights come from a state-dict in the reference key layout
 (`decoder.*`, `post_quant_conv.*`, and — when present — `encoder.*`, `quant_conv.*`).  The encoder reuses the
@@ -16,9 +17,10 @@ at a time as the pipeline does):
     conv's input buffer behind its 2-frame causal halo
   * mid-block attention -> 1x1x1 convs for q/k/out, `pf_gemm_bf16` for V^T, QK^T and PV, `pf_softmax_rows`
   * temporal chunking = the reference's feature cache (C:126-143): each 3x3x3 conv keeps the last two frames of its padded
-    input and they become the halo of the next chunk; chunking is exact, so the chunk length is a memory knob only.
-Spatial tiling (V:468-519) is reproduced by decoding tiles independently and cross-fading them (`tile_sample_min_size`),
-but on 180 GB the un-tiled path is the default unless `enable_tiling()` was called, as in the reference.
+    input and they become the halo of the next chunk (the encoder's stride-2 temporal down-samplers take only the last
+    one, C:140-141); chunking is exact, so the chunk length is a memory knob only.
+Spatial tiling (decode V:468-519, encode V:409-466) is reproduced by running tiles independently and cross-fading them
+(`tile_sample_min_size`), but the un-tiled path is the default unless `enable_tiling()` was called, as in the reference.
 """
 from __future__ import annotations
 
@@ -112,6 +114,7 @@ class B200CausalVAE(torch.nn.Module):
         self._cp = None                     # (group, rank, world) when context-parallel decode is on
         self._cp_ctx = None
         self.cp_frames_per_round = 4        # latent frames per rank per round (memory knob: ~6 GiB per frame at 768p)
+        self.encode_tile_overlap_factor = 0.25
         self.decode_tile_overlap_factor = 0.25
         dev = torch.device(device)
         self._dev = dev
@@ -238,11 +241,13 @@ class B200CausalVAE(torch.nn.Module):
             d.residual, d.res_t_total, d.res_t_offset = residual.data_ptr(), residual.shape[0], res_t_offset
         _lib.check(_lib.load().pf_causal_conv3d(C.byref(d), _lib.stream_ptr()), "pf_causal_conv3d")
 
-    def _halo(self, cv: _Conv, buf: torch.Tensor, first: bool) -> None:
+    def _halo(self, cv: _Conv, buf: torch.Tensor, first: bool) -> torch.Tensor:
         """Fill the 2 leading frames of a 3x3x3 conv's input buffer from its cache (zeros for the first chunk) and
-        remember the last 2 frames of the padded input for the next chunk (reference C:126-143)."""
+        remember the last 2 frames of the padded input for the next chunk (reference C:126-143).  Returns the conv's
+        input: `buf`, except for a later chunk of a stride-2 temporal down-sampler, which takes only the last cached frame
+        as context (C:140-141) so that its stride-2 windows fall where the whole-clip conv puts them: `buf[1:]`."""
         if cv.kt == 1:
-            return
+            return buf
         if self._cp is not None:
             # ring of rounds: my halo = the last two (padded) input frames of the rank before me in this round; rank 0 takes
             # the zero pad in round 0 and afterwards what the LAST rank sent it during the previous round (kept in cv.cache)
@@ -269,12 +274,15 @@ class B200CausalVAE(torch.nn.Module):
                 work.wait()
             if nxt is not None:
                 cv.cache = nxt
-            return
-        if first or cv.cache is None:
+            return buf
+        fresh = first or cv.cache is None
+        if fresh:
             buf[:2].zero_()
         else:
             buf[:2].copy_(cv.cache)
         cv.cache = buf[-2:].clone()
+        stride_t = getattr(cv, "stride", (1, 1, 1))[0]      # a halo'd conv without a stride attribute is stride 1
+        return buf if fresh or stride_t == 1 else buf[1:]
 
     def _gn(self, name: str, x: torch.Tensor, y: torch.Tensor, y_t_offset: int, silu: bool) -> None:
         """x [T, H, W, C] -> y [Ty, H, W, C] frames [y_t_offset, y_t_offset + T)."""
@@ -407,22 +415,34 @@ class B200CausalVAE(torch.nn.Module):
         self._conv(co, a, t, h, w, out=out, store_channels=cfg.out_channels, out_f32=2 if u8 else 1)
         return out
 
-    # ---- encoder (i2v image latent, P:911) ----------------------------------------------------------------------------
-    def _encode_sample(self, x: torch.Tensor) -> torch.Tensor:
-        """x: [1, C, T, H, W] (T = 1 + 8k, H and W multiples of 8) -> moments fp32 [T', h, w, 2*latent], whole clip as one
-        chunk (CausalVaeEncoder.forward D:149-198 with is_init_image=True, then quant_conv V:301)."""
+    # ---- encoder (i2v image latent P:911, training latents P:573-596) -------------------------------------------------
+    @staticmethod
+    def chunk_frame_split(n_frames: int, window_size: int):
+        """chunk_encode's schedule (V:314-327) as frame ranges [a, b): the first chunk takes the image frame plus
+        `window_size` frames, every later chunk `window_size` frames, and the last one whatever is left."""
+        b = min(n_frames, window_size + 1)
+        bounds = [(0, b)]
+        while b < n_frames:
+            bounds.append((b, min(n_frames, b + window_size)))
+            b = bounds[-1][1]
+        return bounds
+
+    def _encode_sample(self, x: torch.Tensor, first: bool = True) -> torch.Tensor:
+        """x: [1, C, T, H, W], ONE chunk (T = 1 + 8k for the first chunk, 8k for a later one; H and W multiples of 8) ->
+        moments fp32 [T', h, w, 2*latent] (CausalVaeEncoder.forward D:149-198, then quant_conv V:301).  Every causal conv
+        takes its halo from the previous chunk's cache unless `first`."""
         cfg, dev = self.cfg, self.device
         _, cx, t, h, w = x.shape
         n_blocks = len(cfg.enc_block_out_channels)
         n_sp, n_tp = sum(cfg.enc_spatial_down_sample), sum(cfg.enc_temporal_down_sample)
         assert h % (1 << n_sp) == 0 and w % (1 << n_sp) == 0, "height / width must be divisible by the spatial down-sampling"
-        assert (t - 1) % (1 << n_tp) == 0, "frames must be 1 + k * temporal down-sampling (V:315)"
+        assert (t - int(first)) % (1 << n_tp) == 0, "frames must be 1 + k * temporal down-sampling (V:315)"
         cin = self.convs["encoder.conv_in"]
         a = torch.empty(t + 2, h, w, cin.cin_p, device=dev, dtype=torch.bfloat16)
-        xx = x if x.dtype in (torch.float32, torch.bfloat16) else x.float()
-        _lib.check(_lib.load().pf_pack_latent(xx.contiguous().data_ptr(), int(xx.dtype == torch.float32), 1, cx, t, h, w,
+        xx = (x if x.dtype in (torch.float32, torch.bfloat16) else x.float()).contiguous()   # a chunk / tile is a strided view
+        _lib.check(_lib.load().pf_pack_latent(xx.data_ptr(), int(xx.dtype == torch.float32), 1, cx, t, h, w,
                                               a.data_ptr(), cin.cin_p, t + 2, 2, None, None, _lib.stream_ptr()), "pf_pack_latent")
-        self._halo(cin, a, True)
+        self._halo(cin, a, first)
         y = torch.empty(t, h, w, cin.cout_p, device=dev, dtype=torch.bfloat16)
         self._conv(cin, a, t, h, w, out=y)                                        # conv_in, D:152
         del a
@@ -431,12 +451,12 @@ class B200CausalVAE(torch.nn.Module):
             xb = None
             for j in range(cfg.enc_layers_per_block[i]):
                 last = j == cfg.enc_layers_per_block[i] - 1
-                y = self._resnet(f"encoder.down_blocks.{i}.resnets.{j}", y, True, halo_out=last and (sp or tp))
+                y = self._resnet(f"encoder.down_blocks.{i}.resnets.{j}", y, first, halo_out=last and (sp or tp))
                 if last and (sp or tp):
                     xb = y                                  # [t+2, h, w, c]: data in frames [2:]
             if sp:                                          # CausalDownsample2x: 3x3x3, stride (1,2,2), K:532-534
                 cv = self.convs[f"encoder.down_blocks.{i}.downsamplers.0.conv"]
-                self._halo(cv, xb, True)
+                self._halo(cv, xb, first)
                 off = 2 if tp else 0
                 h, w = h // 2, w // 2
                 y = torch.empty(t + off, h, w, cv.cout_p, device=dev, dtype=torch.bfloat16)
@@ -445,40 +465,93 @@ class B200CausalVAE(torch.nn.Module):
                 y = y[off:]
             if tp:                                          # CausalTemporalDownsample2x: 3x3x3, stride (2,1,1), K:536-538
                 cv = self.convs[f"encoder.down_blocks.{i}.temporal_downsamplers.0.conv"]
-                self._halo(cv, xb, True)
-                t_out = (t - 1) // 2 + 1                    # padded length t+2, kernel 3, stride 2
+                xin = self._halo(cv, xb, first)             # t+2 frames (zero / cached pair), or t+1 (one cached frame)
+                t_out = (xin.shape[0] - 3) // 2 + 1         # kernel 3, stride 2
                 y = torch.empty(t_out, h, w, cv.cout_p, device=dev, dtype=torch.bfloat16)
-                self._conv(cv, xb[: 2 * (t_out - 1) + 3], t_out, h, w, out=y)
+                self._conv(cv, xin[: 2 * (t_out - 1) + 3], t_out, h, w, out=y)
                 t = t_out
-        y = self._resnet("encoder.mid_block.resnets.0", y, True)
+        y = self._resnet("encoder.mid_block.resnets.0", y, first)
         y = self._mid_attention(y, "encoder")
-        y = self._resnet("encoder.mid_block.resnets.1", y, True)
+        y = self._resnet("encoder.mid_block.resnets.1", y, first)
         co, qc = self.convs["encoder.conv_out"], self.convs["quant_conv"]
         a = torch.empty(t + 2, h, w, y.shape[-1], device=dev, dtype=torch.bfloat16)
         self._gn("encoder.conv_norm_out", y, a, 2, True)
-        self._halo(co, a, True)
+        self._halo(co, a, first)
         m = torch.zeros(t, h, w, qc.cin_p, device=dev, dtype=torch.bfloat16)      # padded channels must read as zero
         self._conv(co, a, t, h, w, out=m, store_channels=co.cout)                 # conv_out -> 2*latent channels
         out = torch.empty(t, h, w, qc.cout, device=dev, dtype=torch.float32)
         self._conv(qc, m, t, h, w, out=out, store_channels=qc.cout, out_f32=True)  # quant_conv (1x1x1), V:301
-        self._reset_caches()
         return out
+
+    def _encode_clip(self, x: torch.Tensor, window: int) -> torch.Tensor:
+        """chunk_encode (V:311-341) for one sample [1, C, T, H, W] -> fp32 [T', h, w, 2*latent]; a window of T or more
+        frames encodes the clip as one chunk (the un-chunked encoder, V:300-301)."""
+        self._reset_caches()
+        try:
+            outs = [self._encode_sample(x[:, :, a:b], i == 0)
+                    for i, (a, b) in enumerate(self.chunk_frame_split(x.shape[2], window))]
+        finally:
+            self._reset_caches()
+        return torch.cat(outs, 0) if len(outs) > 1 else outs[0]
+
+    def _tiled_encode(self, x: torch.Tensor, window: int, tile_sample_min_size: int) -> torch.Tensor:
+        """tiled_encode (V:409-466): pixel tiles encoded independently, their fp32 moments [B, 2C, T', h, w] cross-faded
+        with the tile above and to the left, cropped to the row limit and concatenated."""
+        tile_latent = int(tile_sample_min_size / self.cfg.downsample_scale)
+        overlap = int(tile_sample_min_size * (1 - self.encode_tile_overlap_factor))
+        extent = int(tile_latent * self.encode_tile_overlap_factor)
+        limit = tile_latent - extent
+        rows = []
+        for i in range(0, x.shape[3], overlap):
+            row = []
+            for j in range(0, x.shape[4], overlap):
+                tile = x[:, :, :, i:i + tile_sample_min_size, j:j + tile_sample_min_size]
+                outs = [self._encode_clip(tile[b:b + 1], window) for b in range(x.shape[0])]
+                row.append(torch.stack(outs, 0).permute(0, 4, 1, 2, 3).contiguous())
+            rows.append(row)
+        result_rows = []
+        for i, row in enumerate(rows):
+            res = []
+            for j, tile in enumerate(row):
+                if i > 0:
+                    tile = _blend(rows[i - 1][j], tile, extent, 3)
+                if j > 0:
+                    tile = _blend(row[j - 1], tile, extent, 4)
+                res.append(tile[:, :, :, :limit, :limit])
+            result_rows.append(torch.cat(res, dim=4))
+        return torch.cat(result_rows, dim=3)
 
     @torch.no_grad()
     def encode(self, x: torch.Tensor, return_dict: bool = True, is_init_image: bool = True, temporal_chunk: bool = False,
                window_size: int = 16, tile_sample_min_size: int = 256):
-        """CausalVideoVAE.encode (V:274-308), un-tiled and un-chunked (the pipeline encodes ONE image, P:911; chunking is
-        exact in the reference, so a clip is encoded whole): returns `.latent_dist` with mean / logvar / std / sample()."""
+        """CausalVideoVAE.encode (V:274-308): returns `.latent_dist` with mean / logvar / std / sample().
+
+        As in the reference, with `enable_tiling()` and H or W larger than `tile_sample_min_size` the clip is encoded in
+        overlapping tiles (tiled_encode, V:409-466); otherwise, with `temporal_chunk`, in chunks of `window_size` frames
+        after the first `window_size + 1` (chunk_encode, V:311-341), each causal conv carrying its halo from one chunk to
+        the next; else as one chunk.  Tiles are chunked too when `temporal_chunk` is set.  Chunking is exact: the chunked
+        moments equal the whole-clip ones bit for bit, so `window_size` only bounds the activation memory.  It must be a
+        positive multiple of the temporal down-sampling factor (8 by default): the reference silently misaligns the
+        stride-2 windows of any other window."""
+        tf = 2 ** sum(bool(d) for d in self.cfg.enc_temporal_down_sample)
+        if temporal_chunk and not (isinstance(window_size, int) and window_size > 0 and window_size % tf == 0):
+            raise ValueError(f"window_size={window_size!r} must be a positive multiple of the temporal down-sampling "
+                             f"factor {tf}")
         _lib.require_device()
         assert self.has_encoder, "this B200CausalVAE was built from a state-dict without encoder.* weights"
         assert is_init_image, "clips start with the image frame"
         x = x.to(self.device)
+        window = window_size if temporal_chunk else x.shape[2]
         saved_cp, self._cp = self._cp, None
         try:
-            moments = torch.stack([self._encode_sample(x[i:i + 1]) for i in range(x.shape[0])], 0)   # [B, T', h, w, 2C]
+            if self.use_tiling and (x.shape[-1] > tile_sample_min_size or x.shape[-2] > tile_sample_min_size):
+                moments = self._tiled_encode(x, window, tile_sample_min_size)                       # [B, 2C, T', h, w]
+            else:
+                moments = torch.stack([self._encode_clip(x[i:i + 1], window) for i in range(x.shape[0])], 0)
+                moments = moments.permute(0, 4, 1, 2, 3)                                            # [B, 2C, T', h, w]
         finally:
             self._cp = saved_cp
-        dist = DiagonalGaussian(moments.permute(0, 4, 1, 2, 3).to(self.dtype))
+        dist = DiagonalGaussian(moments.to(self.dtype))
         if not return_dict:
             return (dist,)
         return EncoderOutput(dist)
