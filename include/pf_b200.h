@@ -12,6 +12,8 @@
  * S = diffusion_schedulers/scheduling_flow_matching.py, C = video_vae/modeling_causal_conv.py,
  * R = video_vae/modeling_resnet.py, K = video_vae/modeling_block.py, D = video_vae/modeling_enc_dec.py,
  * V = video_vae/modeling_causal_vae.py.
+ * The text-encoder entries cite transformers 5.5 by class and method: T5 = transformers/models/t5/modeling_t5.py,
+ * CLIP = transformers/models/clip/modeling_clip.py.
  */
 #ifndef PF_B200_H_
 #define PF_B200_H_
@@ -117,7 +119,14 @@ enum {
   PF_EPI_STORE_F32 = 2,  /* out_f32  = acc + bias                     (embedders into the fp32 residual stream) */
   PF_EPI_GATE_RESID = 3, /* out_f32 += gate[b, n] * (acc + bias)      (B:1019-1020, 1027-1028, 1032-1039, 937-938) */
   PF_EPI_QKV_ROPE = 4,   /* N = 3*H*hd: bias, RMSNorm(q,k) per head, RoPE(q,k); head-major Q/K/V stores */
-  PF_EPI_QKV_GELU = 5    /* N = 3*H*hd + n_mlp: columns < n_split as QKV_ROPE, the rest as GELU_BF16 (single block, B:923-936) */
+  PF_EPI_QKV_GELU = 5,   /* N = 3*H*hd + n_mlp: columns < n_split as QKV_ROPE, the rest as GELU_BF16 (single block, B:923-936) */
+  /* text encoders (appended; 0-5 keep their meaning) */
+  PF_EPI_GEGLU_BF16 = 6,      /* T5 T5DenseGatedActDense.forward with gelu_new: W = wi_0 and wi_1 interleaved in 64-row blocks,
+                               * so in every 128-column tile column j < 64 is the gate and j + 64 the linear term;
+                               * out_bf16[r, out_col_begin + tile*64 + j] = gelu_tanh(gate + bias) * (lin + bias).  The output is
+                               * n/2 wide.  Requires n % 128 == 0; never runs on the 128 x 64 kernel (kernel_variant 2 is refused). */
+  PF_EPI_QUICK_GELU_BF16 = 7, /* out_bf16 = x * sigmoid(1.702 x), x = acc + bias  (CLIP-L hidden_act "quick_gelu", CLIPMLP.forward) */
+  PF_EPI_GELU_ERF_BF16 = 8    /* out_bf16 = 0.5 x (1 + erf(x / sqrt 2))            (CLIP-G hidden_act "gelu", CLIPMLP.forward) */
 };
 
 typedef struct pf_gemm_desc {
@@ -170,7 +179,8 @@ PF_API int pf_gemm_bf16(const pf_gemm_desc* desc, void* stream);
  *
  * pf_gemm_fp8: the pf_gemm_bf16 descriptor with d->a, d->w pointing to e4m3 data (lda counts elements = bytes);
  * a_row_scale fp32 [batches, rows_per_batch] indexed like A's rows, w_col_scale fp32 [n].  Requires n % 128 == 0,
- * k % 16 == 0, lda % 16 == 0, kernel_variant 0 and no peer stores (peer_count 0). */
+ * k % 16 == 0, lda % 16 == 0, kernel_variant 0 and no peer stores (peer_count 0).  The text-encoder epilogues (6-8) are
+ * bf16 only: pf_gemm_fp8 refuses them. */
 PF_API int pf_gemm_fp8(const pf_gemm_desc* desc, const float* a_row_scale, const float* w_col_scale, void* stream);
 /* pf_ln_modulate with an e4m3 output: the fp32 LN-modulated row is quantised directly (one rounding) with the contract above;
  * y_fp8 row stride = dim; row_scale fp32 [batches, rows_per_batch] (rows outside the range are not written). */
@@ -352,6 +362,45 @@ PF_API int pf_pack_latent(const void* z, int32_t z_is_f32, int32_t b, int32_t c,
  * blended axis: b[o, y, i] = a[o, la - extent + y, i] * (1 - y/extent) + b[o, y, i] * (y/extent) for y < extent (in place). */
 PF_API int pf_blend_tiles(const float* a, float* b, int64_t outer, int32_t la, int32_t lb, int64_t inner, int32_t extent,
                           void* stream);
+
+/* ------------------------------------------------------------------ text encoders (T5 v1.1 encoder, CLIP text transformer)
+ * The GEMMs run on pf_gemm_bf16: the packed q|k|v projection and CLIPTextModelWithProjection's text_projection on
+ * STORE_BF16, the residual adds after the attention output projection and the MLP down-projection on GATE_RESID with a ones
+ * gate into an fp32 residual stream, the MLP up-projection on GEGLU (T5) / QUICK_GELU (CLIP-L) / GELU_ERF (CLIP-G).  CLIP's
+ * LayerNorms (CLIPEncoderLayer.forward, CLIPTextTransformer.forward final_layer_norm) run on pf_ln_modulate with
+ * shift = bias, scale = weight - 1 and mod_batch_stride = 0.
+ *
+ * Short-sequence attention: T5Attention.forward (scores + position_bias + the T5Stack.forward additive key mask, fp32
+ * softmax) and CLIPAttention.forward (causal, scale head_dim^-0.5):
+ *   out[b, q, h*64 + :] = softmax_k(scale * Q[b,q,h] . K[b,k,h] + bias[h, k - q + seq - 1] + mask(b, q, k)) . V[b,k,h]
+ *   mask = -inf where key_mask[b, k] == 0 (for every query row, padded rows included, as under T5's additive mask),
+ *          or causal && k > q.
+ * qkv: bf16 [batch * seq, ld_qkv], q of head h at columns [64 h, +64), k at 64 (heads + h), v at 64 (2 heads + h) (the packed
+ * QKV GEMM output).  out: bf16 [batch * seq, ldo].  bias: fp32 [heads, 2 seq - 1] (T5Attention.compute_bias as a Toeplitz
+ * table) or NULL; key_mask: int32 [batch, seq] or NULL.  seq <= 256, head_dim 64.  A batch whose key mask is all zeros has
+ * no defined result (the host wrapper refuses it); such a row is written as zeros. */
+typedef struct pf_attn_text_desc {
+  const void* qkv;
+  int64_t ld_qkv;
+  void* out;
+  int64_t ldo;
+  int32_t batch, heads, seq, head_dim;
+  float scale;
+  const float* bias;
+  const int32_t* key_mask;
+  int32_t causal;
+} pf_attn_text_desc;
+PF_API int pf_attn_fwd_text(const pf_attn_text_desc* desc, void* stream);
+/* T5LayerNorm.forward: y_bf16[r, :] = x[r, :] * rsqrt(mean(x[r, :]^2) + eps) * w  (w fp32 [dim]), for rows
+ * [row_begin, row_begin + row_count) of each batch of x fp32 [batches, rows_per_batch, dim]; y has x's row layout. */
+PF_API int pf_rms_norm_rows(const float* x, void* y_bf16, const float* w, int32_t batches, int32_t rows_per_batch,
+                            int32_t row_begin, int32_t row_count, int32_t dim, float eps, void* stream);
+/* Embedding lookup (T5Stack.forward embed_tokens, no scaling; CLIPTextEmbeddings.forward token + position):
+ * out_f32[r, :] = table[ids[r], :] (+ pos_table[r % rows_per_batch, :]), ids int32 [rows], table bf16 [vocab, dim], pos_table
+ * bf16 [max_pos, dim] or NULL.  The host validates ids against vocab; the kernel never reads outside the table (an id out of
+ * range gives a zero row). */
+PF_API int pf_embed_tokens(const int32_t* ids, int64_t rows, int32_t rows_per_batch, const void* table, int32_t vocab,
+                           int32_t dim, const void* pos_table, int32_t max_pos, float* out_f32, void* stream);
 
 #ifdef __cplusplus
 }

@@ -24,10 +24,12 @@ SYMBOLS = [
     "pf_ctx_create", "pf_ctx_destroy", "pf_ctx_record_begin", "pf_ctx_record_end", "pf_ctx_replay", "pf_dit_step_flux",
     "pf_dit_step_mmdit", "pf_vae_decode_chunk",
     "pf_peer_alloc", "pf_peer_free", "pf_peer_export", "pf_peer_open", "pf_peer_close", "pf_peer_barrier", "pf_peer_bcast",
+    "pf_attn_fwd_text", "pf_rms_norm_rows", "pf_embed_tokens",
 ]
 
 PF_OPT_GEMM_STAGED_RESID, PF_OPT_GEMM_WAVE_TILING, PF_OPT_ATTN_PAIR_KERNEL, PF_OPT_ATTN_TILE_PHASE, PF_OPT_ATTN_TRIPLE_KERNEL = range(5)
 PF_EPI_STORE_BF16, PF_EPI_GELU_BF16, PF_EPI_STORE_F32, PF_EPI_GATE_RESID, PF_EPI_QKV_ROPE, PF_EPI_QKV_GELU = range(6)
+PF_EPI_GEGLU_BF16, PF_EPI_QUICK_GELU_BF16, PF_EPI_GELU_ERF_BF16 = range(6, 9)
 
 
 class GemmDesc(C.Structure):
@@ -61,6 +63,14 @@ class AttnDesc(C.Structure):
         ("peer_out", C.c_void_p * 8),
         ("peer_count", C.c_int32), ("peer_chunk_rows", C.c_int32), ("peer_col_begin", C.c_int32),
         ("group_sched", C.c_void_p), ("group_mask_index", C.c_void_p), ("group_mask_bits", C.c_void_p),
+    ]
+
+
+class AttnTextDesc(C.Structure):
+    _fields_ = [
+        ("qkv", C.c_void_p), ("ld_qkv", C.c_int64), ("out", C.c_void_p), ("ldo", C.c_int64),
+        ("batch", C.c_int32), ("heads", C.c_int32), ("seq", C.c_int32), ("head_dim", C.c_int32),
+        ("scale", C.c_float), ("bias", C.c_void_p), ("key_mask", C.c_void_p), ("causal", C.c_int32),
     ]
 
 
@@ -151,6 +161,11 @@ def load() -> C.CDLL:
     lib.pf_softmax_rows.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_float, C.c_void_p]
     lib.pf_pack_latent.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.pf_attn_fwd_text.argtypes = [C.POINTER(AttnTextDesc), C.c_void_p]
+    lib.pf_rms_norm_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                     C.c_float, C.c_void_p]
+    lib.pf_embed_tokens.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
+                                    C.c_void_p, C.c_void_p]
     _lib = lib
     return lib
 

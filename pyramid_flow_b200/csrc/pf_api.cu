@@ -133,6 +133,7 @@ int num_sms() {
 int warmup_gemm();
 int warmup_conv();
 int warmup_attn();
+int warmup_text();
 
 }  // namespace pf
 
@@ -242,11 +243,12 @@ int pf_warmup(void) {
   int rc = pf::warmup_gemm();
   if (!rc) rc = pf::warmup_conv();
   if (!rc) rc = pf::warmup_attn();
+  if (!rc) rc = pf::warmup_text();
   return rc;
 }
 
 const char* pf_last_error(void) { return pf::g_err; }
-int pf_version(void) { return 201; }
+int pf_version(void) { return 202; }
 int64_t pf_launch_count(void) { return pf::g_launches.load(); }
 
 int pf_device_check(void) {

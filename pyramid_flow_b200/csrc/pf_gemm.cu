@@ -13,7 +13,8 @@
 // The producer runs ahead into the next tile's stages while the consumers are in the epilogue.
 //
 // Epilogues (include/pf_b200.h PF_EPI_*): bias / GELU-tanh / fp32 store / gate*x+residual / per-head RMSNorm + RoPE
-// with head-major Q,K,V stores / the single-block fused q|k|v|mlp split.
+// with head-major Q,K,V stores / the single-block fused q|k|v|mlp split; for the text encoders GEGLU (gate and linear
+// columns 64 apart in every 128-wide tile, half-width output), quick-GELU and exact (erf) GELU.
 // pf_gemm_fp8 runs the cluster kernel on e4m3 operands: 128 x 128 tiles (one 64-row half per consumer warpgroup), K = 128
 // per stage, per-stage promotion of the fp8 partial sums into fp32, and the same epilogues after the per-row x per-column
 // dequantisation scale.
@@ -63,6 +64,18 @@ constexpr int BK = PIPE_BK;
 constexpr double GEMM_RATE_CLUSTER = 1.25;
 constexpr double GEMM_RATE_128 = 1.0;
 constexpr double GEMM_RATE_64 = 0.75;
+
+// the bf16-output activations of the single-column epilogues (GELU_BF16, QKV_GELU's mlp part, QUICK_GELU, GELU_ERF)
+template <int EPI>
+__device__ __forceinline__ float epi_act(float x) {
+  if constexpr (EPI == PF_EPI_GELU_BF16 || EPI == PF_EPI_QKV_GELU) return gelu_tanh_f(x);
+  if constexpr (EPI == PF_EPI_QUICK_GELU_BF16) return x * rcp_approx_f(1.0f + ex2_approx_f(-1.702f * 1.4426950408889634f * x));
+  if constexpr (EPI == PF_EPI_GELU_ERF_BF16) return 0.5f * x * (1.0f + erff(x * 0.7071067811865476f));
+  return x;
+}
+constexpr bool epi_is_act_bf16(int epi) {
+  return epi == PF_EPI_GELU_BF16 || epi == PF_EPI_QUICK_GELU_BF16 || epi == PF_EPI_GELU_ERF_BF16;
+}
 
 // ---- epilogue helpers (one thread == one output row) -----------------------
 __device__ __forceinline__ void store_bf16x32(__nv_bfloat16* dst, const float (&x)[32]) {
@@ -178,7 +191,16 @@ __device__ __forceinline__ void epilogue_tile(const GemmArgs& g, const float* ac
   bool qkv_tile = (EPI == PF_EPI_QKV_ROPE);
   if (EPI == PF_EPI_QKV_GELU) qkv_tile = n_base < g.n_split;
 
-  if (qkv_tile) {
+  if constexpr (EPI == PF_EPI_GEGLU_BF16) {
+    // gate columns [32 half, +32) of the tile, linear columns 64 further; output columns n_base / 2 + 32 half + [0, 32)
+    static_assert(BN == 128, "GEGLU runs on 128-wide tiles only");
+    float x[32], lin[32];
+    load_bias32(x, srow + 32 * half, g.bias ? g.bias + n_base + 32 * half : nullptr);
+    load_bias32(lin, srow + 64 + 32 * half, g.bias ? g.bias + n_base + 64 + 32 * half : nullptr);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) x[i] = gelu_tanh_f(x[i]) * lin[i];
+    if (valid) store_bf16x32(reinterpret_cast<__nv_bfloat16*>(g.out) + out_row * g.ldo + g.out_col_begin + n_base / 2 + 32 * half, x);
+  } else if (qkv_tile) {
     const int pos = g.out_row_begin + m;
 #pragma unroll 1
     for (int h = half; h < BN / 64; h += 2) qkv_head_epilogue(g, srow + h * 64, n_base + h * 64, b, pos, valid);
@@ -211,12 +233,12 @@ __device__ __forceinline__ void epilogue_tile(const GemmArgs& g, const float* ac
       const int n0 = n_base + c * 32;
       float x[32];
       load_bias32(x, srow + c * 32, g.bias ? g.bias + n0 : nullptr);
-      if (EPI == PF_EPI_GELU_BF16 || EPI == PF_EPI_QKV_GELU) {
+      if (epi_is_act_bf16(EPI) || EPI == PF_EPI_QKV_GELU) {
 #pragma unroll
-        for (int i = 0; i < 32; ++i) x[i] = gelu_tanh_f(x[i]);
+        for (int i = 0; i < 32; ++i) x[i] = epi_act<EPI>(x[i]);
       }
       if (!valid) continue;
-      if (EPI == PF_EPI_STORE_BF16 || EPI == PF_EPI_GELU_BF16 || EPI == PF_EPI_QKV_GELU) {
+      if (EPI == PF_EPI_STORE_BF16 || epi_is_act_bf16(EPI) || EPI == PF_EPI_QKV_GELU) {
         const int col = (EPI == PF_EPI_QKV_GELU) ? (g.out_col_begin + n0 - g.n_split) : (g.out_col_begin + n0);
         store_bf16x32(reinterpret_cast<__nv_bfloat16*>(g.out) + out_row * g.ldo + col, x);
       } else if (EPI == PF_EPI_STORE_F32) {
@@ -460,7 +482,31 @@ __device__ __forceinline__ void epilogue_frag(const GemmArgs& g, const float (&a
     }
   };
 
-  if (qkv_tile) {
+  if constexpr (EPI == PF_EPI_GEGLU_BF16) {
+    // column group i < 8 is the gate, i + 8 the linear term of the same thread: output column n_base / 2 + 8 i + c_thr
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int n = n_base + 8 * i + c_thr;
+      float2 bg = make_float2(0.f, 0.f), bl = make_float2(0.f, 0.f);
+      if (g.bias != nullptr) {
+        bg = __ldg(reinterpret_cast<const float2*>(g.bias + n));
+        bl = __ldg(reinterpret_cast<const float2*>(g.bias + n + 64));
+      }
+#pragma unroll
+      for (int hr = 0; hr < 2 * H; ++hr) {
+        const int h = hr >> 1, half = hr & 1;
+        const int m = m_base + r_thr + 64 * h + 8 * half;
+        const float2 ga = value2(hr, 4 * i + 2 * half, n);
+        const float2 la = value2(hr, 4 * (i + 8) + 2 * half, n + 64);
+        const float x0 = gelu_tanh_f(ga.x + bg.x) * (la.x + bl.x);
+        const float x1 = gelu_tanh_f(ga.y + bg.y) * (la.y + bl.y);
+        if (m >= g.row_count) continue;
+        const size_t out_row = static_cast<size_t>(b) * g.out_batch_rows + g.out_row_begin + m;
+        *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(g.out) + out_row * g.ldo + g.out_col_begin + n_base / 2 + 8 * i +
+                                     c_thr) = pack_bf16x2(x0, x1);
+      }
+    }
+  } else if (qkv_tile) {
     const int inner = g.heads * g.head_dim;
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {   // the tile's two 64-column heads
@@ -574,9 +620,9 @@ __device__ __forceinline__ void epilogue_frag(const GemmArgs& g, const float (&a
         const float2 a = value2(hr, 4 * i + 2 * half, n);
         float x0 = a.x + bb.x;
         float x1 = a.y + bb.y;
-        if (EPI == PF_EPI_GELU_BF16 || EPI == PF_EPI_QKV_GELU) {
-          x0 = gelu_tanh_f(x0);
-          x1 = gelu_tanh_f(x1);
+        if (epi_is_act_bf16(EPI) || EPI == PF_EPI_QKV_GELU) {
+          x0 = epi_act<EPI>(x0);
+          x1 = epi_act<EPI>(x1);
         }
         if (m >= g.row_count) continue;
         const size_t out_row = static_cast<size_t>(b) * g.out_batch_rows + g.out_row_begin + m;
@@ -748,18 +794,23 @@ static int dispatch_tile(int tile, const CUtensorMap& tm_a, const CUtensorMap& t
   switch (tile) {
     case 0: return launch_cluster<EPI>(tm_a, tm_b, g, stream);
     case 128: return launch_gemm<128, EPI>(tm_a, tm_b, g, stream);
-    case 64: return launch_gemm<64, EPI>(tm_a, tm_b, g, stream);
+    case 64:
+      if constexpr (EPI != PF_EPI_GEGLU_BF16) return launch_gemm<64, EPI>(tm_a, tm_b, g, stream);
+      break;
   }
   set_error("unsupported GEMM tile %d", tile);
   return -1;
 }
 
+// the text-encoder epilogues (> QKV_GELU) have no fp8 instantiation, and GEGLU none on the 128 x 64 kernel
 template <int EPI>
 static int warm_epi() {
   int rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_cluster_kernel<EPI, false>), Cfg16::SMEM_BYTES, "gemm cluster");
-  if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_cluster_kernel<EPI, true>), Cfg8::SMEM_BYTES, "gemm cluster fp8");
+  if constexpr (EPI <= PF_EPI_QKV_GELU)
+    if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_cluster_kernel<EPI, true>), Cfg8::SMEM_BYTES, "gemm cluster fp8");
   if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_bf16_wgmma_kernel<128, EPI>), PipeCfg<128>::SMEM_BYTES, "gemm<128>");
-  if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_bf16_wgmma_kernel<64, EPI>), PipeCfg<64>::SMEM_BYTES, "gemm<64>");
+  if constexpr (EPI != PF_EPI_GEGLU_BF16)
+    if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_bf16_wgmma_kernel<64, EPI>), PipeCfg<64>::SMEM_BYTES, "gemm<64>");
   return rc;
 }
 // load every instantiation and set its dynamic-smem attribute on the current device (so nothing initialises inside a
@@ -771,6 +822,9 @@ int warmup_gemm() {
   if (!rc) rc = warm_epi<PF_EPI_GATE_RESID>();
   if (!rc) rc = warm_epi<PF_EPI_QKV_ROPE>();
   if (!rc) rc = warm_epi<PF_EPI_QKV_GELU>();
+  if (!rc) rc = warm_epi<PF_EPI_GEGLU_BF16>();
+  if (!rc) rc = warm_epi<PF_EPI_QUICK_GELU_BF16>();
+  if (!rc) rc = warm_epi<PF_EPI_GELU_ERF_BF16>();
   if (!rc) rc = cluster_slots() > 0 ? 0 : -1;
   return rc;
 }
@@ -789,7 +843,10 @@ static int gemm_args_from_desc(const pf_gemm_desc* d, const char* fn, int k_alig
   PF_REQUIRE((reinterpret_cast<uintptr_t>(d->a) & 15) == 0 && (reinterpret_cast<uintptr_t>(d->w) & 15) == 0,
              "%s: operands must be 16-byte aligned", fn);
   const int epi = d->epilogue;
-  PF_REQUIRE(epi >= 0 && epi <= PF_EPI_QKV_GELU, "%s: unknown epilogue %d", fn, epi);
+  PF_REQUIRE(epi >= 0 && epi <= PF_EPI_GELU_ERF_BF16, "%s: unknown epilogue %d", fn, epi);
+  if (epi == PF_EPI_GEGLU_BF16)
+    PF_REQUIRE(d->n % 128 == 0 && d->kernel_variant != 2,
+               "%s: GEGLU needs n %% 128 == 0 (n=%d) and 128-wide tiles (kernel_variant %d)", fn, d->n, d->kernel_variant);
 
   // The QKV epilogues work per 64-column head, so any multiple of 64 is head-aligned.
   const bool qkv = (epi == PF_EPI_QKV_ROPE || epi == PF_EPI_QKV_GELU);
@@ -889,8 +946,9 @@ extern "C" int pf_gemm_bf16(const pf_gemm_desc* d, void* stream_) {
     const long long waves64 = (d->batches * mt128 * (d->n / 64) + sms - 1) / sms;
     const double cost0 = waves0 * 2.0 / GEMM_RATE_CLUSTER, cost128 = waves128 * 1.0 / GEMM_RATE_128,
                  cost64 = waves64 * 0.5 / GEMM_RATE_64;
-    if (cost128 < cost0 && cost128 <= cost64) tile = 128;
-    else if (cost64 < cost0) tile = 64;
+    const bool allow64 = epi != PF_EPI_GEGLU_BF16;   // GEGLU pairs columns 64 apart inside a 128-wide tile
+    if (cost128 < cost0 && (cost128 <= cost64 || !allow64)) tile = 128;
+    else if (allow64 && cost64 < cost0) tile = 64;
   }
   if (tile != 0) bn = tile;
   const int tile_rows = tile == 0 ? CBM : BM;
@@ -924,6 +982,9 @@ extern "C" int pf_gemm_bf16(const pf_gemm_desc* d, void* stream_) {
     case PF_EPI_GATE_RESID: return dispatch_tile<PF_EPI_GATE_RESID>(tile, tm_a, tm_b, g, stream);
     case PF_EPI_QKV_ROPE: return dispatch_tile<PF_EPI_QKV_ROPE>(tile, tm_a, tm_b, g, stream);
     case PF_EPI_QKV_GELU: return dispatch_tile<PF_EPI_QKV_GELU>(tile, tm_a, tm_b, g, stream);
+    case PF_EPI_GEGLU_BF16: return dispatch_tile<PF_EPI_GEGLU_BF16>(tile, tm_a, tm_b, g, stream);
+    case PF_EPI_QUICK_GELU_BF16: return dispatch_tile<PF_EPI_QUICK_GELU_BF16>(tile, tm_a, tm_b, g, stream);
+    case PF_EPI_GELU_ERF_BF16: return dispatch_tile<PF_EPI_GELU_ERF_BF16>(tile, tm_a, tm_b, g, stream);
   }
   return -1;
 }
@@ -937,6 +998,7 @@ extern "C" int pf_gemm_fp8(const pf_gemm_desc* d, const float* a_row_scale, cons
   PF_REQUIRE(d->kernel_variant == 0, "pf_gemm_fp8: kernel_variant %d: there is one fp8 kernel (0)", d->kernel_variant);
   PF_REQUIRE(d->n % 128 == 0, "pf_gemm_fp8: n=%d must be a multiple of 128", d->n);
   PF_REQUIRE(d->epilogue != PF_EPI_QKV_GELU || d->n_split % 128 == 0, "pf_gemm_fp8: QKV_GELU needs n_split %% 128 == 0");
+  PF_REQUIRE(d->epilogue <= PF_EPI_QKV_GELU, "pf_gemm_fp8: epilogue %d is bf16 only (pf_gemm_bf16)", d->epilogue);
   GemmArgs g;
   if (int rc = gemm_args_from_desc(d, "pf_gemm_fp8", 16, g)) return rc;
   g.a_scale = a_row_scale;

@@ -10,7 +10,7 @@ from typing import Optional
 import torch
 
 from . import _lib
-from ._lib import (AttnDesc, GemmDesc, PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_GELU,
+from ._lib import (AttnDesc, AttnTextDesc, GemmDesc, PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_GELU,
                    PF_EPI_QKV_ROPE, PF_EPI_STORE_BF16, PF_EPI_STORE_F32)
 
 
@@ -346,3 +346,50 @@ def attn_fwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tenso
             assert g3.sched.shape[-1] == sched.shape[-1]
             d.group_sched, d.group_mask_index, d.group_mask_bits = g3.sched.data_ptr(), g3.mask_index.data_ptr(), g3.mask_bits.data_ptr()
     _lib.check(_lib.load().pf_attn_fwd_masked(C.byref(d), _lib.stream_ptr()), "pf_attn_fwd_masked")
+
+
+def attn_fwd_text(qkv: torch.Tensor, out: torch.Tensor, *, batch: int, heads: int, seq: int, scale: float,
+                  bias: Optional[torch.Tensor] = None, key_mask: Optional[torch.Tensor] = None, causal: bool = False) -> None:
+    """Short-sequence attention of the text encoders (pf_attn_fwd_text): qkv bf16 [batch * seq, >= 3 * heads * 64] (q | k | v
+    per head, row stride qkv.stride(0)) -> out bf16 [batch * seq, >= heads * 64].  bias fp32 [heads, 2 seq - 1] (T5 relative
+    position bias as a Toeplitz table), key_mask int32 [batch, seq] on the device (0 removes the key for every query)."""
+    assert qkv.dtype == torch.bfloat16 and out.dtype == torch.bfloat16 and qkv.is_cuda and out.is_cuda
+    assert qkv.stride(-1) == 1 and out.stride(-1) == 1 and qkv.shape[0] == batch * seq and out.shape[0] == batch * seq
+    d = AttnTextDesc()
+    d.qkv, d.ld_qkv, d.out, d.ldo = qkv.data_ptr(), qkv.stride(0), out.data_ptr(), out.stride(0)
+    d.batch, d.heads, d.seq, d.head_dim = batch, heads, seq, 64
+    d.scale = scale
+    if bias is not None:
+        assert bias.dtype == torch.float32 and bias.is_contiguous() and tuple(bias.shape) == (heads, 2 * seq - 1)
+    if key_mask is not None:
+        assert key_mask.dtype == torch.int32 and key_mask.is_contiguous() and tuple(key_mask.shape) == (batch, seq)
+    d.bias, d.key_mask, d.causal = _ptr(bias), _ptr(key_mask), int(causal)
+    _lib.check(_lib.load().pf_attn_fwd_text(C.byref(d), _lib.stream_ptr()), "pf_attn_fwd_text")
+
+
+def rms_norm_rows(x: torch.Tensor, y: torch.Tensor, w: torch.Tensor, *, batches: int = 1, rows_per_batch: Optional[int] = None,
+                  row_begin: int = 0, row_count: Optional[int] = None, eps: float = 1e-6) -> None:
+    """T5LayerNorm: x fp32 [.., dim] -> y bf16 (same row layout) = x * rsqrt(mean(x^2) + eps) * w (pf_rms_norm_rows)."""
+    assert x.dtype == torch.float32 and y.dtype == torch.bfloat16 and w.dtype == torch.float32
+    assert x.is_contiguous() and y.is_contiguous() and w.is_contiguous() and x.shape == y.shape
+    dim = x.shape[-1]
+    if rows_per_batch is None:
+        rows_per_batch = x.numel() // (dim * batches)
+    if row_count is None:
+        row_count = rows_per_batch - row_begin
+    _lib.check(_lib.load().pf_rms_norm_rows(x.data_ptr(), y.data_ptr(), w.data_ptr(), batches, rows_per_batch, row_begin, row_count,
+                                            dim, eps, _lib.stream_ptr()), "pf_rms_norm_rows")
+
+
+def embed_tokens(ids: torch.Tensor, table: torch.Tensor, out: torch.Tensor, *, rows_per_batch: int,
+                 pos_table: Optional[torch.Tensor] = None) -> None:
+    """out fp32 [rows, dim] = table[ids] (+ pos_table[row % rows_per_batch]) (pf_embed_tokens); ids int32 [rows] on the device."""
+    assert ids.dtype == torch.int32 and ids.is_contiguous() and table.dtype == torch.bfloat16 and table.is_contiguous()
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.shape == (ids.numel(), table.shape[1])
+    max_pos = 0
+    if pos_table is not None:
+        assert pos_table.dtype == torch.bfloat16 and pos_table.is_contiguous() and pos_table.shape[1] == table.shape[1]
+        max_pos = pos_table.shape[0]
+    _lib.check(_lib.load().pf_embed_tokens(ids.data_ptr(), ids.numel(), rows_per_batch, table.data_ptr(), table.shape[0],
+                                           table.shape[1], _ptr(pos_table), max_pos, out.data_ptr(), _lib.stream_ptr()),
+               "pf_embed_tokens")

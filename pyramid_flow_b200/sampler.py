@@ -2,7 +2,8 @@
 
 Mirrors `PyramidDiTForVideoGeneration.generate` / `generate_i2v` (P:791-1003) / `generate_one_unit` / `get_pyramid_latent` / `sample_block_noise` /
 `decode_latent` (pyramid_dit/pyramid_dit_for_video_gen_pipeline.py:1006-1219, 706-788, 555-570, 697-703, 1221-1243) from
-the point where text embeddings exist (text encoders are out of scope).  In a reference checkout the
+the point where text embeddings exist (the prompt encoders run on the library too, as
+`pyramid_flow_b200.text_encoder.B200FluxTextEncoder` / `B200SD3TextEncoder`).  In a reference checkout the
 pipeline itself stays the call surface (INTEGRATION.md); this mirror is what tests and bench.py drive on the GPU, and
 it is pinned against the unmodified reference loop by tests/golden/sampler_small.pt (oracle/pin/make_golden.py).
 
