@@ -229,6 +229,10 @@ typedef struct pf_attn_desc {
   const int32_t* group_sched;
   const int32_t* group_mask_index;
   const void* group_mask_bits;
+  /* optional (NULL = not written): fp32 [batch, heads, seq], each row's log-sum-exp of the SCALED scores in natural log,
+   * lse[q] = ln sum_kv exp(scale * q.k) over the allowed kv (+inf for a row without one); what pf_attn_bwd_masked takes.
+   * Whole local launches only: refused with peer_count > 1 or q_row_begin != 0.  Without it the kernel runs unchanged. */
+  float* lse;
 } pf_attn_desc;
 
 /* Host helper: from host copies of seg/time ids builds, for each (batch, 128-row q tile), the list of 128-wide kv
@@ -264,6 +268,46 @@ PF_API int64_t pf_attn_build_group_masks(const int32_t* seg_host, const int32_t*
                                          const int32_t* pair_sched_host /* or NULL */,
                                          const int32_t* pair_mask_index_host /* or NULL */);
 PF_API int pf_attn_fwd_masked(const pf_attn_desc* desc, void* stream);
+/* Host helper: the kv-major transpose of a pf_attn_build_schedule schedule, for the backward's dK / dV pass.  For each
+ * (batch, 128-row kv tile) it lists, in increasing order, the q tiles whose row of tile_sched_host names this kv tile, with the
+ * same partial flag.  Row layout: [count, (q_tile << 1) | needs_mask, ...], sched_stride int32 per row (the stride of the q
+ * schedule, >= 1 + ceil(seq/128)); `out` holds batch * ceil(seq/128) rows. */
+PF_API int pf_attn_build_kv_schedule(const int32_t* tile_sched_host, int32_t batch, int32_t seq, int32_t sched_stride,
+                                     int32_t* out);
+
+/* ------------------------------------------------------------------ masked joint attention backward (wgmma + TMA)
+ * Gradients of out = softmax(Q K^T * scale + mask) V with the mask of pf_attn_fwd_masked, replacing the autograd backward of
+ * F.scaled_dot_product_attention with the dense [B,1,S,S] bool mask that the reference's training path runs in every block
+ * (VarlenSelfAttentionWithT5Mask B:363-365, VarlenSelfAttnSingle B:596-598; the mask built by merge_input F:341-350).
+ * With P = exp(scale * Q K^T - lse) on the allowed pairs (0 elsewhere) and delta[q] = sum_d dO[q, d] O[q, d]:
+ *   dV = P^T dO,   dS = P o (dO V^T - delta),   dQ = scale * dS K,   dK = scale * dS^T Q.
+ * Three launches, no atomics (the result is deterministic): delta (one warp per row), dK / dV (one CTA per (b, h, kv tile),
+ * q tiles streamed in the order of kv_sched) and dQ (one CTA per (b, h, q tile), kv tiles in the order of tile_sched).
+ * Operands bf16, every product and sum in fp32; head_dim 64, any seq (rows past seq are neither read as data nor stored). */
+typedef struct pf_attn_bwd_desc {
+  const void* q;       /* bf16 [batch, heads, seq, 64] */
+  const void* k;
+  const void* v;
+  const void* out;     /* bf16 [batch, seq, heads*64]: the forward's output; row stride ldo, batch stride out_batch_stride */
+  int64_t ldo, out_batch_stride;
+  const void* dout;    /* bf16 [batch, seq, heads*64]: the gradient of out; row stride lddo, batch stride dout_batch_stride
+                        * (a view: e.g. the stage slice of a gradient whose rows hold more than one stage, so its batch stride
+                        * is not seq * lddo).  Strides in elements, multiples of 8; row strides >= heads*64. */
+  int64_t lddo, dout_batch_stride;
+  const float* lse;    /* fp32 [batch, heads, seq] from pf_attn_fwd_masked */
+  int32_t batch, heads, seq, head_dim;
+  float scale;
+  const int32_t* seg;        /* device [batch, seq] */
+  const int32_t* time;       /* device [batch, seq] */
+  const int32_t* tile_sched; /* device, pf_attn_build_schedule */
+  const int32_t* kv_sched;   /* device, pf_attn_build_kv_schedule (same sched_stride) */
+  int32_t sched_stride;
+  float* delta;              /* workspace fp32 [batch, heads, seq] */
+  void* dq;                  /* bf16 [batch, heads, seq, 64] */
+  void* dk;
+  void* dv;
+} pf_attn_bwd_desc;
+PF_API int pf_attn_bwd_masked(const pf_attn_bwd_desc* desc, void* stream);
 
 /* ------------------------------------------------------------------ LayerNorm + AdaLN modulate pre-pass (HBM-bound)
  * y_bf16[r, :] = LN(x_f32[r, :], eps) * (1 + scale[b, :]) + shift[b, :]   (N:174, N:234, N:120, B:1022-1023, B:1035-1036)

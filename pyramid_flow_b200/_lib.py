@@ -17,7 +17,7 @@ SYMBOLS = [
     "pf_last_error", "pf_version", "pf_device_check", "pf_warmup", "pf_set_option", "pf_get_option", "pf_launch_count",
     "pf_gemm_bf16", "pf_gemm_fp8", "pf_ln_modulate_fp8", "pf_quantize_rows_fp8",
     "pf_attn_build_schedule", "pf_attn_build_pair_schedule", "pf_attn_build_pair_masks", "pf_attn_build_group_schedule",
-    "pf_attn_build_group_masks", "pf_attn_fwd_masked",
+    "pf_attn_build_group_masks", "pf_attn_fwd_masked", "pf_attn_build_kv_schedule", "pf_attn_bwd_masked",
     "pf_ln_modulate", "pf_small_linear", "pf_timestep_embedding",
     "pf_patchify", "pf_unpatchify", "pf_cfg_euler_step", "pf_stage_hop",
     "pf_causal_conv3d", "pf_groupnorm_stats", "pf_groupnorm_apply", "pf_softmax_rows", "pf_pack_latent", "pf_blend_tiles",
@@ -63,6 +63,20 @@ class AttnDesc(C.Structure):
         ("peer_out", C.c_void_p * 8),
         ("peer_count", C.c_int32), ("peer_chunk_rows", C.c_int32), ("peer_col_begin", C.c_int32),
         ("group_sched", C.c_void_p), ("group_mask_index", C.c_void_p), ("group_mask_bits", C.c_void_p),
+        ("lse", C.c_void_p),
+    ]
+
+
+class AttnBwdDesc(C.Structure):
+    _fields_ = [
+        ("q", C.c_void_p), ("k", C.c_void_p), ("v", C.c_void_p),
+        ("out", C.c_void_p), ("ldo", C.c_int64), ("out_batch_stride", C.c_int64),
+        ("dout", C.c_void_p), ("lddo", C.c_int64), ("dout_batch_stride", C.c_int64), ("lse", C.c_void_p),
+        ("batch", C.c_int32), ("heads", C.c_int32), ("seq", C.c_int32), ("head_dim", C.c_int32),
+        ("scale", C.c_float),
+        ("seg", C.c_void_p), ("time", C.c_void_p), ("tile_sched", C.c_void_p), ("kv_sched", C.c_void_p),
+        ("sched_stride", C.c_int32),
+        ("delta", C.c_void_p), ("dq", C.c_void_p), ("dk", C.c_void_p), ("dv", C.c_void_p),
     ]
 
 
@@ -119,6 +133,8 @@ def load() -> C.CDLL:
     lib.pf_quantize_rows_fp8.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int32,
                                          C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     lib.pf_attn_fwd_masked.argtypes = [C.POINTER(AttnDesc), C.c_void_p]
+    lib.pf_attn_bwd_masked.argtypes = [C.POINTER(AttnBwdDesc), C.c_void_p]
+    lib.pf_attn_build_kv_schedule.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     lib.pf_attn_build_schedule.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     lib.pf_attn_build_pair_schedule.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     lib.pf_attn_build_pair_masks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,

@@ -40,8 +40,12 @@ struct AttnArgs {
   // sequence parallel: output rows go straight into the owning rank's buffer (pf_b200.h)
   __nv_bfloat16* peer_out[PF_MAX_PEERS];
   int peer_count, peer_chunk_rows, peer_col_begin;
+  // fp32 [batch, heads, seq]: natural-log log-sum-exp of each row's scaled scores (the attention backward's softmax statistic)
+  float* lse;
 };
 
+// kLse: also store each row's log-sum-exp.  A template flag, so the launches without it run exactly the code they always ran.
+template <bool kLse>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                 const __grid_constant__ CUtensorMap tm_v, const AttnArgs a) {
@@ -241,6 +245,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     const float inv = (l > 0.f) ? 1.f / l : 0.f;
     const int qpos = qt * ATT_BM + row0 + 8 * r;
     if (qpos >= a.seq) continue;
+    if constexpr (kLse) {
+      // lse = scale * max + ln(sum exp(scale * (s - max))) = ln 2 * (max * scale * log2 e + log2 l); +inf for a row without an
+      // allowed score, so that the backward's exp(s * scale - lse) is 0 there
+      if (t4 == 0) a.lse[static_cast<size_t>(bh) * a.seq + qpos] = (l > 0.f) ? (m_run[r] * c + log2f(l)) * 0.6931471805599453f : INFINITY;
+    }
     __nv_bfloat16* dst;
     if (a.peer_count > 1) {
       const int pr = qpos / a.peer_chunk_rows;
@@ -254,8 +263,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   }
 }
 
+int warmup_attn_bwd();
+
 int warmup_attn() {
-  return ensure_dyn_smem(reinterpret_cast<const void*>(attn_fwd_kernel), ATT_SMEM_BYTES, "attn_fwd_kernel");
+  int rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_fwd_kernel<false>), ATT_SMEM_BYTES, "attn_fwd_kernel");
+  if (!rc) rc = ensure_dyn_smem(reinterpret_cast<const void*>(attn_fwd_kernel<true>), ATT_SMEM_BYTES, "attn_fwd_kernel<lse>");
+  if (!rc) rc = warmup_attn_bwd();
+  return rc;
 }
 
 }  // namespace pf
@@ -341,6 +355,10 @@ extern "C" int pf_attn_fwd_masked(const pf_attn_desc* d, void* stream_) {
                d->peer_chunk_rows, d->seq);
     for (int i = 0; i < d->peer_count; ++i) PF_REQUIRE(d->peer_out[i] != nullptr, "pf_attn_fwd_masked: peer_out[%d] is null", i);
   }
+  if (d->lse != nullptr)
+    PF_REQUIRE(d->peer_count <= 1 && d->q_row_begin == 0,
+               "pf_attn_fwd_masked: lse is computed for whole local launches only (peer_count %d, q_row_begin %d)", d->peer_count,
+               d->q_row_begin);
   CUtensorMap tm[3];
   const void* ptrs[3] = {d->q, d->k, d->v};
   for (int i = 0; i < 3; ++i) {
@@ -367,10 +385,14 @@ extern "C" int pf_attn_fwd_masked(const pf_attn_desc* d, void* stream_) {
   a.peer_chunk_rows = d->peer_chunk_rows;
   a.peer_col_begin = d->peer_col_begin;
   for (int i = 0; i < PF_MAX_PEERS; ++i) a.peer_out[i] = static_cast<__nv_bfloat16*>(d->peer_out[i]);
+  a.lse = d->lse;
 
   if (int rc = warmup_attn()) return rc;
   // q tile index = q_tiles - 1 - blockIdx.x: a shorter grid.x drops the leading (lowest) q tiles
   dim3 grid(q_tiles - d->q_row_begin / ATT_BM, d->heads, d->batch);
-  attn_fwd_kernel<<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tm[0], tm[1], tm[2], a);
+  if (a.lse != nullptr)
+    attn_fwd_kernel<true><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tm[0], tm[1], tm[2], a);
+  else
+    attn_fwd_kernel<false><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tm[0], tm[1], tm[2], a);
   return check_launch("pf_attn_fwd_masked");
 }

@@ -224,3 +224,32 @@ extern "C" int64_t pf_attn_build_group_masks(const int32_t* seg, const int32_t* 
   }
   return blocks;
 }
+
+// Host helper: the kv-major transpose of the q-tile schedule (pf_b200.h pf_attn_build_kv_schedule).  Walking the q tiles in
+// increasing order appends each q tile to the rows of the kv tiles it names, so every kv row comes out sorted by q tile.
+extern "C" int pf_attn_build_kv_schedule(const int32_t* tile_sched, int32_t batch, int32_t seq, int32_t sched_stride,
+                                         int32_t* out) {
+  using namespace pf;
+  PF_REQUIRE(tile_sched && out && batch > 0 && seq > 0, "pf_attn_build_kv_schedule: bad arguments");
+  const int tiles = (seq + 127) / 128;
+  PF_REQUIRE(sched_stride >= 1 + tiles, "pf_attn_build_kv_schedule: stride %d too small", sched_stride);
+  for (int b = 0; b < batch; ++b) {
+    int32_t* rows = out + static_cast<size_t>(b) * tiles * sched_stride;
+    for (int i = 0; i < tiles * sched_stride; ++i) rows[i] = 0;
+    for (int qt = 0; qt < tiles; ++qt) {
+      const int32_t* row = tile_sched + (static_cast<size_t>(b) * tiles + qt) * sched_stride;
+      PF_REQUIRE(row[0] >= 0 && row[0] <= tiles, "pf_attn_build_kv_schedule: bad count %d (batch %d, q tile %d)", row[0], b, qt);
+      for (int e = 0; e < row[0]; ++e) {
+        const int kt = row[1 + e] >> 1;
+        PF_REQUIRE(kt >= 0 && kt < tiles, "pf_attn_build_kv_schedule: kv tile %d out of range (batch %d, q tile %d)", kt, b, qt);
+        int32_t* kr = rows + static_cast<size_t>(kt) * sched_stride;
+        // a well-formed q schedule names a kv tile at most once per q row, so a kv row never holds more than `tiles` entries
+        PF_REQUIRE(kr[0] < tiles && kr[0] < sched_stride - 1 && (kr[0] == 0 || (kr[kr[0]] >> 1) != qt),
+                   "pf_attn_build_kv_schedule: kv tile %d named more than once by a q tile (batch %d, q tile %d)", kt, b, qt);
+        kr[1 + kr[0]] = (qt << 1) | (row[1 + e] & 1);
+        ++kr[0];
+      }
+    }
+  }
+  return 0;
+}

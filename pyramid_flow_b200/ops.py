@@ -10,7 +10,7 @@ from typing import Optional
 import torch
 
 from . import _lib
-from ._lib import (AttnDesc, AttnTextDesc, GemmDesc, PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_GELU,
+from ._lib import (AttnBwdDesc, AttnDesc, AttnTextDesc, GemmDesc, PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_GELU,
                    PF_EPI_QKV_ROPE, PF_EPI_STORE_BF16, PF_EPI_STORE_F32)
 
 
@@ -310,11 +310,24 @@ def attn_build_group_schedule(sched: torch.Tensor, seq: int, seg: torch.Tensor, 
     return PairSchedule(gs, midx, bits)
 
 
+def attn_build_kv_schedule(sched: torch.Tensor, seq: int) -> torch.Tensor:
+    """Tile schedule (int32 CPU [batch, q_tiles, stride], attn_build_schedule) -> its kv-major transpose, int32 CPU
+    [batch, kv_tiles, stride]: per kv tile [count, (q_tile << 1) | needs_mask, ...] (pf_attn_build_kv_schedule)."""
+    sched = sched.to(torch.int32).contiguous().cpu()
+    batch, tiles, stride = sched.shape
+    out = torch.zeros(batch, tiles, stride, dtype=torch.int32)
+    _lib.check(_lib.load().pf_attn_build_kv_schedule(sched.data_ptr(), batch, seq, stride, out.data_ptr()),
+               "pf_attn_build_kv_schedule")
+    return out
+
+
 def attn_fwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tensor, seg: torch.Tensor,
              time: torch.Tensor, sched: torch.Tensor, scale: float, variant: int = 0, q_row_begin: int = 0,
-             pair_sched: Optional[PairSchedule] = None, ldo: Optional[int] = None, peer: Optional[dict] = None) -> None:
+             pair_sched: Optional[PairSchedule] = None, ldo: Optional[int] = None, peer: Optional[dict] = None,
+             lse: Optional[torch.Tensor] = None) -> None:
     """q,k,v bf16 [B,H,S,64]; out bf16 [B,S,*] (row stride = out.stride(1)); seg/time/sched int32 on device.
-    Only q rows >= q_row_begin (multiple of 128) are computed; other rows of `out` are left untouched."""
+    Only q rows >= q_row_begin (multiple of 128) are computed; other rows of `out` are left untouched.
+    lse: optional fp32 [B,H,S], filled with each row's natural-log log-sum-exp of the scaled scores (for attn_bwd)."""
     assert q.dtype == torch.bfloat16 and q.is_contiguous() and k.is_contiguous() and v.is_contiguous()
     b, h, s, hd = q.shape
     d = AttnDesc()
@@ -345,7 +358,46 @@ def attn_fwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tenso
             assert g3.sched.is_contiguous() and g3.mask_index.is_contiguous() and g3.mask_bits.is_contiguous()
             assert g3.sched.shape[-1] == sched.shape[-1]
             d.group_sched, d.group_mask_index, d.group_mask_bits = g3.sched.data_ptr(), g3.mask_index.data_ptr(), g3.mask_bits.data_ptr()
+    if lse is not None:
+        assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (b, h, s)
+        d.lse = lse.data_ptr()
     _lib.check(_lib.load().pf_attn_fwd_masked(C.byref(d), _lib.stream_ptr()), "pf_attn_fwd_masked")
+
+
+def attn_bwd_rows_ok(t: torch.Tensor) -> bool:
+    """Whether a bf16 [B, S, >=H*64] tensor can be handed to attn_bwd as it is (pf_attn_bwd_masked's layout rules: unit
+    column stride, row and batch strides multiples of 8 elements, 16-byte aligned)."""
+    return (t.dtype == torch.bfloat16 and t.ndim == 3 and t.stride(2) == 1 and t.stride(1) % 8 == 0 and t.stride(0) % 8 == 0
+            and t.stride(1) >= t.shape[2] and t.stride(0) > 0 and t.data_ptr() % 16 == 0)
+
+
+def attn_bwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor,
+             seg: torch.Tensor, time: torch.Tensor, sched: torch.Tensor, kv_sched: torch.Tensor, scale: float,
+             dq: torch.Tensor, dk: torch.Tensor, dv: torch.Tensor, delta: Optional[torch.Tensor] = None) -> None:
+    """Gradients of attn_fwd (pf_attn_bwd_masked): q,k,v,dq,dk,dv bf16 [B,H,S,64]; out/dout bf16 [B,S,>=H*64], any views
+    that satisfy attn_bwd_rows_ok (their row and batch strides are passed); lse fp32 [B,H,S] from attn_fwd;
+    seg/time/sched/kv_sched int32 on the device."""
+    b, h, s, hd = q.shape
+    for t in (q, k, v, dq, dk, dv):
+        assert t.dtype == torch.bfloat16 and t.is_cuda and t.is_contiguous() and tuple(t.shape) == (b, h, s, hd)
+    for t in (out, dout):
+        assert t.is_cuda and tuple(t.shape[:2]) == (b, s) and t.shape[2] >= h * hd, (tuple(t.shape), (b, s, h * hd))
+        assert attn_bwd_rows_ok(t), f"attn_bwd: layout {tuple(t.stride())} not supported, pass a contiguous copy"
+    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (b, h, s)
+    assert sched.shape == kv_sched.shape and sched.dtype == torch.int32 and kv_sched.dtype == torch.int32
+    if delta is None:
+        delta = torch.empty(b, h, s, dtype=torch.float32, device=q.device)
+    d = AttnBwdDesc()
+    d.q, d.k, d.v = q.data_ptr(), k.data_ptr(), v.data_ptr()
+    d.out, d.ldo, d.out_batch_stride = out.data_ptr(), out.stride(1), out.stride(0)
+    d.dout, d.lddo, d.dout_batch_stride = dout.data_ptr(), dout.stride(1), dout.stride(0)
+    d.lse = lse.data_ptr()
+    d.batch, d.heads, d.seq, d.head_dim = b, h, s, hd
+    d.scale = scale
+    d.seg, d.time, d.tile_sched, d.kv_sched = seg.data_ptr(), time.data_ptr(), sched.data_ptr(), kv_sched.data_ptr()
+    d.sched_stride = sched.shape[-1]
+    d.delta, d.dq, d.dk, d.dv = delta.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr()
+    _lib.check(_lib.load().pf_attn_bwd_masked(C.byref(d), _lib.stream_ptr()), "pf_attn_bwd_masked")
 
 
 def attn_fwd_text(qkv: torch.Tensor, out: torch.Tensor, *, batch: int, heads: int, seq: int, scale: float,

@@ -1,0 +1,253 @@
+"""Trainable masked attention, and its drop-in for the reference's autoregressive training path.
+
+`masked_attention(q, k, v, seg, time, scale)` is softmax attention under mask(q, kv) = (seg[q] == seg[kv]) &&
+(time[q] >= time[kv]) with a backward: the forward is pf_attn_fwd_masked (which also stores each row's log-sum-exp), the
+backward pf_attn_bwd_masked (include/pf_b200.h).  Gradients are taken w.r.t. the bf16 q / k / v with fp32 accumulation, and are
+deterministic (no atomics), so a forward recomputed under torch.utils.checkpoint gives the bits of the first one.
+
+`install_training_attention(ref_dit)` puts it under an unmodified reference `PyramidFluxTransformer` instance, trained with
+`use_flash_attn=False` (scripts/train_pyramid_flow.sh without --use_flash_attn): the `varlen_attn` callable of every
+FluxAttnProcessor2_0 / FluxSingleAttnProcessor2_0 (VarlenSelfAttentionWithT5Mask B:328-376, VarlenSelfAttnSingle B:568-606)
+is replaced by a library callable with the same signature and output layout, and the instance's `merge_input` (F:239-352)
+is wrapped so that each stage's dense [B, 1, S, S] bool mask (F:341-350) becomes a `StageAttentionPlan` carrying that stage's
+seg / time ids and tile schedules.  No reference source changes; `uninstall_training_attention` restores the instance.
+"""
+from __future__ import annotations
+
+import sys
+from typing import Dict, Optional, Tuple
+
+import torch
+
+from . import _lib, ops
+
+HEAD_DIM = 64
+
+
+class StageAttentionPlan:
+    """One stage's attention mask in the form the kernels take: seg / time int32 [B, S] on the device, the q-tile schedule
+    (pf_attn_build_schedule) and its kv-major transpose (pf_attn_build_kv_schedule), both on the device."""
+
+    def __init__(self, seg: torch.Tensor, time: torch.Tensor, sched: torch.Tensor, kv_sched: torch.Tensor):
+        self.seg, self.time, self.sched, self.kv_sched = seg, time, sched, kv_sched
+
+    @property
+    def shape(self) -> Tuple[int, int]:
+        return tuple(self.seg.shape)
+
+
+_PLANS: Dict[tuple, StageAttentionPlan] = {}
+_PLAN_CACHE_SIZE = 32
+
+
+def plan_for(seg: torch.Tensor, time: torch.Tensor, device=None) -> StageAttentionPlan:
+    """The StageAttentionPlan of seg / time ids [B, S] (any integer dtype, any device), cached by their content: a training
+    run sees a handful of stage layouts, so after the first steps this costs one small device-to-host copy."""
+    device = torch.device(device) if device is not None else seg.device
+    seg_c = seg.detach().to("cpu", torch.int32).contiguous()
+    time_c = time.detach().to("cpu", torch.int32).contiguous()
+    assert seg_c.ndim == 2 and seg_c.shape == time_c.shape, (seg_c.shape, time_c.shape)
+    key = (str(device), tuple(seg_c.shape), seg_c.numpy().tobytes(), time_c.numpy().tobytes())
+    plan = _PLANS.get(key)
+    if plan is None:
+        sched, _ = ops.attn_build_schedule(seg_c, time_c)
+        kv_sched = ops.attn_build_kv_schedule(sched, seg_c.shape[1])
+        plan = StageAttentionPlan(seg_c.to(device), time_c.to(device), sched.to(device), kv_sched.to(device))
+        if len(_PLANS) >= _PLAN_CACHE_SIZE:
+            _PLANS.clear()
+        _PLANS[key] = plan
+    return plan
+
+
+class _MaskedAttention(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, q, k, v, plan: StageAttentionPlan, scale: float):
+        b, h, s, hd = q.shape
+        out = torch.empty(b, s, h * hd, dtype=torch.bfloat16, device=q.device)
+        lse = torch.empty(b, h, s, dtype=torch.float32, device=q.device)
+        ops.attn_fwd(q, k, v, out, plan.seg, plan.time, plan.sched, scale, lse=lse)
+        ctx.save_for_backward(q, k, v, out, lse)
+        ctx.plan, ctx.scale = plan, scale
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        q, k, v, out, lse = ctx.saved_tensors
+        plan = ctx.plan
+        dout = dout.to(torch.bfloat16)
+        # a stage's slice of a wider gradient (the single blocks' cat along the sequence, then with the MLP branch) arrives
+        # as a view with its own row and batch strides: passed as they are when the kernels can address them
+        if not ops.attn_bwd_rows_ok(dout):
+            dout = dout.contiguous()
+        dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+        ops.attn_bwd(q, k, v, out, dout, lse, plan.seg, plan.time, plan.sched, plan.kv_sched, ctx.scale, dq, dk, dv)
+        return dq, dk, dv, None, None
+
+
+def _check_qkv(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor) -> None:
+    if q.shape[-1] != HEAD_DIM:
+        raise ValueError(f"masked_attention: head_dim {q.shape[-1]} unsupported (the kernels are written for {HEAD_DIM})")
+    if not (q.shape == k.shape == v.shape) or q.ndim != 4:
+        raise ValueError(f"masked_attention: q, k, v must all be [B, H, S, {HEAD_DIM}] (got {q.shape}, {k.shape}, {v.shape})")
+    if not q.is_cuda:
+        raise RuntimeError("masked_attention runs on the GPU only (pyramid_flow_b200 has no CPU path)")
+
+
+def attend(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, plan: StageAttentionPlan, scale: float) -> torch.Tensor:
+    """q, k, v [B, H, S, 64] (any float dtype; taken to bf16) -> out [B, S, H*64] in q's dtype, under the plan's mask."""
+    _check_qkv(q, k, v)
+    if tuple(plan.shape) != (q.shape[0], q.shape[2]):
+        raise ValueError(f"masked_attention: plan is for [B, S] = {tuple(plan.shape)}, q is {tuple(q.shape)}")
+    _lib.require_device()
+    dt = q.dtype
+    q, k, v = (t.to(torch.bfloat16).contiguous() for t in (q, k, v))
+    out = _MaskedAttention.apply(q, k, v, plan, float(scale))
+    return out if dt == torch.bfloat16 else out.to(dt)
+
+
+def masked_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, seg: torch.Tensor, time: torch.Tensor,
+                     scale: Optional[float] = None) -> torch.Tensor:
+    """softmax(q k^T * scale | mask) v with mask(i, j) = (seg[b, i] == seg[b, j]) && (time[b, i] >= time[b, j]), differentiable
+    w.r.t. q, k, v.  q, k, v: [B, H, S, 64]; seg / time: integer [B, S]; scale defaults to 64 ** -0.5 (SDPA's default).
+    Returns [B, S, H*64] (the layout SDPA's output takes after .transpose(1, 2).flatten(2, 3))."""
+    _check_qkv(q, k, v)
+    scale = q.shape[-1] ** -0.5 if scale is None else scale
+    return attend(q, k, v, plan_for(seg, time, q.device), scale)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# drop-in for the reference training path
+# ----------------------------------------------------------------------------------------------------------------------
+def _stage_plan(attention_mask, i_p: int) -> StageAttentionPlan:
+    plan = attention_mask[i_p] if attention_mask is not None else None
+    if not isinstance(plan, StageAttentionPlan):
+        raise TypeError("the installed training attention takes the StageAttentionPlan objects of the wrapped merge_input, "
+                        f"got {type(plan).__name__} (was the model's merge_input replaced after install_training_attention?)")
+    return plan
+
+
+class _JointAttention:
+    """Stands for VarlenSelfAttentionWithT5Mask (B:328-376): per stage, text tokens of that stage (encoder rows i_p::stages)
+    then its video tokens; the reference's apply_rope; attention under the stage's plan; outputs split back."""
+
+    def __init__(self, apply_rope):
+        self.apply_rope = apply_rope
+
+    def __call__(self, query, key, value, encoder_query, encoder_key, encoder_value, heads, scale, hidden_length=None,
+                 image_rotary_emb=None, attention_mask=None):
+        encoder_length = encoder_query.shape[1]
+        num_stages = len(hidden_length)
+        encoder_qkv = torch.stack([encoder_query, encoder_key, encoder_value], dim=2)   # [bs, sub_seq, 3, head, head_dim]
+        qkv = torch.stack([query, key, value], dim=2)
+        i_sum = 0
+        enc_out, hid_out = [], []
+        for i_p, length in enumerate(hidden_length):
+            plan = _stage_plan(attention_mask, i_p)
+            tokens = torch.cat([encoder_qkv[i_p::num_stages], qkv[:, i_sum:i_sum + length]], dim=1)
+            q, k, v = tokens.unbind(2)                                                   # [bs, tot_seq, nhead, dim]
+            if image_rotary_emb is not None:
+                q, k = self.apply_rope(q, k, image_rotary_emb[i_p])
+            out = attend(q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), plan, q.shape[-1] ** -0.5)
+            enc_out.append(out[:, :encoder_length])
+            hid_out.append(out[:, encoder_length:])
+            i_sum += length
+        # 'b n s d -> (b n) s d'
+        return torch.cat(hid_out, dim=1), torch.stack(enc_out, dim=1).flatten(0, 1)
+
+
+class _SingleAttention:
+    """Stands for VarlenSelfAttnSingle (B:568-606): the single blocks' joint sequence is already stage-major."""
+
+    def __init__(self, apply_rope):
+        self.apply_rope = apply_rope
+
+    def __call__(self, query, key, value, heads, scale, hidden_length=None, image_rotary_emb=None, attention_mask=None):
+        qkv = torch.stack([query, key, value], dim=2)
+        i_sum = 0
+        outs = []
+        for i_p, length in enumerate(hidden_length):
+            plan = _stage_plan(attention_mask, i_p)
+            q, k, v = qkv[:, i_sum:i_sum + length].unbind(2)
+            if image_rotary_emb is not None:
+                q, k = self.apply_rope(q, k, image_rotary_emb[i_p])
+            outs.append(attend(q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), plan, q.shape[-1] ** -0.5))
+            i_sum += length
+        return torch.cat(outs, dim=1)
+
+
+def stage_ids(ref_dit, sample, encoder_attention_mask: torch.Tensor, hidden_length) -> list:
+    """Per stage (seg, time) int32 [B, S_stage] of the reference's mask (F:320-350): seg 1 for valid tokens, 0 for padded
+    text (encoder_attention_mask[i_p::num_stages]); time = the temporal order ids of the model's own
+    _prepare_pyramid_image_ids, 0 for text, or 0 everywhere without use_temporal_causal."""
+    num_stages = len(sample)
+    first = sample[0][-1] if isinstance(sample[0], list) else sample[0]
+    device, pad_bs = first.device, first.shape[0]
+    image_ids = ref_dit._prepare_pyramid_image_ids(sample, pad_bs, device) if ref_dit.use_temporal_causal else None
+    out = []
+    for i_p, length in enumerate(hidden_length):
+        text = (encoder_attention_mask[i_p::num_stages] != 0).to(torch.int32)
+        seg = torch.cat([text, torch.ones(pad_bs, length, dtype=torch.int32, device=text.device)], dim=1)
+        time = torch.zeros_like(seg)
+        if image_ids is not None:
+            time[:, text.shape[1]:] = image_ids[i_p][:, :, 0].to(device=time.device, dtype=torch.int32)
+        out.append((seg, time))
+    return out
+
+
+def _ref_module_attr(obj, name):
+    return getattr(sys.modules[type(obj).__module__], name)
+
+
+def install_training_attention(ref_dit) -> None:
+    """Run every attention of an unmodified reference PyramidFluxTransformer (use_flash_attn=False, no sequence parallelism,
+    head_dim 64) on masked_attention.  Forward values are the reference's up to bf16 rounding inside the attention; the
+    dense masks are no longer built into the saved graph.  Idempotent; undone by uninstall_training_attention."""
+    if getattr(ref_dit, "_pf_training_attention", None) is not None:
+        return
+    if getattr(ref_dit, "use_flash_attn", False):
+        raise ValueError("install_training_attention: the model runs the flash varlen path (use_flash_attn=True), which this "
+                         "does not replace; build it with use_flash_attn=False")
+    if _ref_module_attr(ref_dit, "is_sequence_parallel_initialized")():
+        raise ValueError("install_training_attention: sequence parallelism is initialised; its all-to-all attention path is "
+                         "not replaced")
+    head_dim = ref_dit.config.attention_head_dim
+    if head_dim != HEAD_DIM:
+        raise ValueError(f"install_training_attention: attention_head_dim {head_dim} unsupported ({HEAD_DIM} only)")
+
+    saved = []
+    for m in ref_dit.modules():
+        proc = getattr(m, "processor", None)
+        kind = type(proc).__name__
+        if kind not in ("FluxAttnProcessor2_0", "FluxSingleAttnProcessor2_0"):
+            continue
+        rope = _ref_module_attr(proc, "apply_rope")
+        saved.append((proc, proc.varlen_attn))
+        proc.varlen_attn = _JointAttention(rope) if kind == "FluxAttnProcessor2_0" else _SingleAttention(rope)
+
+    had_own = "merge_input" in ref_dit.__dict__
+    original = ref_dit.merge_input
+
+    def merge_input(sample, encoder_hidden_length, encoder_attention_mask):
+        res = list(original(sample, encoder_hidden_length, encoder_attention_mask))
+        hidden_length = res[1]
+        ids = stage_ids(ref_dit, sample, encoder_attention_mask, hidden_length)
+        res[7] = [plan_for(seg, time) for seg, time in ids]      # the dense masks are dropped here
+        return tuple(res)
+
+    ref_dit.merge_input = merge_input
+    ref_dit._pf_training_attention = (saved, had_own, original)
+
+
+def uninstall_training_attention(ref_dit) -> None:
+    """Restore what install_training_attention changed on the instance."""
+    state = getattr(ref_dit, "_pf_training_attention", None)
+    if state is None:
+        return
+    saved, had_own, original = state
+    for proc, fn in saved:
+        proc.varlen_attn = fn
+    if had_own:
+        ref_dit.merge_input = original
+    else:
+        del ref_dit.merge_input
+    del ref_dit._pf_training_attention
