@@ -386,7 +386,10 @@ PF_API int pf_causal_conv3d(const pf_conv3d_desc* desc, void* stream);
 
 /* per-frame GroupNorm (CausalGroupNorm C:36-43) on channels-last bf16 [frames, voxels, channels]:
  * stats[frame, group] = (mean, rstd); workspace: >= frames * 64 * channels * 2 floats.  Deterministic, and independent of
- * how many frames are passed per call (chunk-invariant). */
+ * how many frames are passed per call (chunk-invariant).  Per-channel sums are taken in fp32 about the frame's first voxel
+ * and combined in double, so a large group mean does not cancel the variance: mean within 1e-5 std + 2^-23 |mean| and
+ * rstd within 1e-5 relative of an fp64 two-pass GroupNorm of the same bf16 input, at |mean|/std up to 100 and frames
+ * up to 768x1280 voxels. */
 PF_API int pf_groupnorm_stats(const void* x_bf16, int32_t frames, int64_t voxels, int32_t channels, int32_t groups,
                               float eps, float* stats, float* workspace, int64_t workspace_floats, void* stream);
 /* y[b, t + y_t_offset, vox, c] = act((x[b, t, vox, c] - mean) * rstd * gamma[c] + beta[c]), act = SiLU if silu

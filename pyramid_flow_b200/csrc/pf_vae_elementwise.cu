@@ -7,7 +7,11 @@
 namespace pf {
 
 // ---------------------------------------------------------------------------------------------------------------
-// GroupNorm statistics, pass 1: per (frame, split) partial sum / sum-of-squares per CHANNEL.
+// GroupNorm statistics, pass 1: per (frame, split) partial sum / sum-of-squares per CHANNEL of x - K, with the pivot
+// K = x[frame, voxel 0, channel].  Unshifted fp32 sums lose the variance to cancellation in E[x^2] - mean^2 once a
+// group's |mean| is large against its std (~4% rstd error at |mean|/std = 100); shifted by a value inside the channel's
+// own distribution they stay accurate.  Every thread reads the same pivot, so the sums remain deterministic and
+// independent of how frames are split across calls.
 // Each thread owns one 8-channel vector position and strides over voxels; 128-bit loads, fp32 partials.
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
@@ -27,14 +31,26 @@ gn_partial_kernel(const __nv_bfloat16* __restrict__ x, long long voxels, int cha
   for (int i = 0; i < 8; ++i) s[i] = ss[i] = 0.f;
   if (vlane < vstep) {
     const __nv_bfloat16* base = x + static_cast<size_t>(frame) * voxels * channels;
+    float k[8];
+    {
+      const uint4 u = __ldg(reinterpret_cast<const uint4*>(base) + cv);
+      const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float2 f = __bfloat1622float2(h[i]);
+        k[2 * i] = f.x;
+        k[2 * i + 1] = f.y;
+      }
+    }
     for (long long v = v0 + vlane; v < v1; v += vstep) {
       const uint4 u = __ldg(reinterpret_cast<const uint4*>(base + v * channels) + cv);
       const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const float2 f = __bfloat1622float2(h[i]);
-        s[2 * i] += f.x; ss[2 * i] += f.x * f.x;
-        s[2 * i + 1] += f.y; ss[2 * i + 1] += f.y * f.y;
+        const float d0 = f.x - k[2 * i], d1 = f.y - k[2 * i + 1];   // exact for bf16 operands within 2^16 of each other
+        s[2 * i] += d0; ss[2 * i] += d0 * d0;
+        s[2 * i + 1] += d1; ss[2 * i + 1] += d1 * d1;
       }
     }
     float* dst = sh + (static_cast<size_t>(vlane) * channels + cv * 8) * 2;
@@ -53,22 +69,29 @@ gn_partial_kernel(const __nv_bfloat16* __restrict__ x, long long voxels, int cha
   }
 }
 
-// pass 2: (mean, rstd) per (frame, group), combined in double
-__global__ void gn_finalize_kernel(const float* __restrict__ partial, int frames, int nsplit, int channels, int groups,
-                                   long long voxels, float eps, float* __restrict__ stats /* [frames, groups, 2] */) {
+// pass 2: (mean, rstd) per (frame, group), combined in double: per channel the shifted sums S = sum(x - K) and
+// SS = sum((x - K)^2) give sum(x) = S + nK and sum(x^2) = SS + 2KS + nK^2
+__global__ void gn_finalize_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ partial, int frames,
+                                   int nsplit, int channels, int groups, long long voxels, float eps,
+                                   float* __restrict__ stats /* [frames, groups, 2] */) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= frames * groups) return;
   const int frame = idx / groups, g = idx - frame * groups;
   const int cpg = channels / groups;
+  const double nv = static_cast<double>(voxels);
   double s = 0.0, ss = 0.0;
-  for (int sp = 0; sp < nsplit; ++sp) {
-    const float* p = partial + ((static_cast<size_t>(frame) * nsplit + sp) * channels + g * cpg) * 2;
-    for (int c = 0; c < cpg; ++c) {
-      s += p[2 * c];
-      ss += p[2 * c + 1];
+  for (int c = g * cpg; c < (g + 1) * cpg; ++c) {
+    double sc = 0.0, ssc = 0.0;
+    for (int sp = 0; sp < nsplit; ++sp) {
+      const float* p = partial + ((static_cast<size_t>(frame) * nsplit + sp) * channels + c) * 2;
+      sc += p[0];
+      ssc += p[1];
     }
+    const double k = __bfloat162float(x[static_cast<size_t>(frame) * voxels * channels + c]);
+    s += sc + nv * k;
+    ss += ssc + 2.0 * k * sc + nv * k * k;
   }
-  const double n = static_cast<double>(voxels) * cpg;
+  const double n = nv * cpg;
   const double mean = s / n;
   double var = ss / n - mean * mean;
   if (var < 0.0) var = 0.0;
@@ -191,6 +214,7 @@ int pf_groupnorm_stats(const void* x, int32_t frames, int64_t voxels, int32_t ch
   using namespace pf;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   PF_REQUIRE(x && stats && workspace, "pf_groupnorm_stats: null pointer");
+  PF_REQUIRE(frames > 0 && voxels > 0 && groups > 0, "pf_groupnorm_stats: bad shape");
   PF_REQUIRE(channels % 8 == 0 && channels % groups == 0 && channels <= 2048, "pf_groupnorm_stats: channels=%d unsupported", channels);
   // the split count depends on the frame SIZE only, never on how many frames are in the call: per-frame statistics are
   // bitwise identical whatever the temporal chunking
@@ -206,8 +230,8 @@ int pf_groupnorm_stats(const void* x, int32_t frames, int64_t voxels, int32_t ch
   int rc = check_launch("pf_groupnorm_stats(partial)");
   if (rc) return rc;
   const int n = frames * groups;
-  gn_finalize_kernel<<<(n + 127) / 128, 128, 0, stream>>>(workspace, frames, static_cast<int>(nsplit), channels, groups,
-                                                          voxels, eps, stats);
+  gn_finalize_kernel<<<(n + 127) / 128, 128, 0, stream>>>(static_cast<const __nv_bfloat16*>(x), workspace, frames,
+                                                          static_cast<int>(nsplit), channels, groups, voxels, eps, stats);
   return check_launch("pf_groupnorm_stats(finalize)");
 }
 
@@ -216,7 +240,7 @@ int pf_groupnorm_apply(const void* x, void* y, int32_t b, int32_t t, int64_t vox
                        int32_t y_t_offset, void* stream) {
   using namespace pf;
   PF_REQUIRE(x && y && stats && gamma && beta, "pf_groupnorm_apply: null pointer");
-  PF_REQUIRE(channels % 8 == 0 && channels % groups == 0, "pf_groupnorm_apply: channels=%d unsupported", channels);
+  PF_REQUIRE(groups > 0 && channels % 8 == 0 && channels % groups == 0, "pf_groupnorm_apply: channels=%d unsupported", channels);
   PF_REQUIRE(y_t_offset >= 0 && y_t_offset + t <= y_t_total, "pf_groupnorm_apply: frame window out of range");
   const long long total = static_cast<long long>(b) * t * voxels * (channels / 8);
   gn_apply_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
