@@ -8,7 +8,7 @@ bench) turn it on.  A model class mixes this in and supplies:
   _forward_eager(clips, timestep_ratio, enc, mask, pooled) -> [velocity]   the host-launched step
   _graph_key_fields() -> tuple        its switches that change the launch sequence (part of the capture key)
   _graph_prealloc(plan, clips)        allocates, outside the capture, everything the step uses (workspace, peer arena)
-  _graph_plan(clips, mask)            (optional) -> (SeqPlan, device tables the step reads that the plan does not hold)
+  plan_for(clip_shapes, mask)         the step's SeqPlan (the capture keeps it, and the device tables it holds, alive)
 """
 from __future__ import annotations
 
@@ -31,13 +31,10 @@ class GraphedStep:
         self.graph_replays = 0          # bookkeeping for bench.py: replays and kernel launches replayed
         self.graph_launches_replayed = 0
 
-    def _graph_plan(self, clips, mask):
-        return self.plan_for([cl.shape for cl in clips], mask), None
-
     def _forward_graphed(self, clips, timestep_ratio, enc, mask, pooled):
         """Replay the step's captured launch sequence; inputs are copied into the capture's static buffers."""
         dev = self.device
-        plan, tables = self._graph_plan(clips, mask)
+        plan = self.plan_for([cl.shape for cl in clips], mask)
         ins = [*clips, timestep_ratio, enc, pooled]
         key = (id(plan), *self._graph_key_fields(), tuple((tuple(x.shape), x.dtype) for x in ins))
         ent = self._graphs.get(key)
@@ -79,9 +76,9 @@ class GraphedStep:
                 finally:
                     graph.capture_end()
             torch.cuda.current_stream().wait_stream(side)
-            # the captured pointers must stay allocated as long as the graph lives: workspaces, plan and plan-side tables
-            ent = dict(graph=graph, static=static, out=out, launches=_lib.launch_count() - n0, plan=plan, tables=tables,
-                       mask=mask, ws=dict(self._ws))
+            # the captured pointers must stay allocated as long as the graph lives: workspaces and plan
+            ent = dict(graph=graph, static=static, out=out, launches=_lib.launch_count() - n0, plan=plan, mask=mask,
+                       ws=dict(self._ws))
             self._graphs[key] = ent
         else:
             for st, x in zip(ent["static"], ins):
