@@ -12,6 +12,17 @@
 //                           softmax (exact running max, exp2) runs on the accumulator fragments, P is re-packed in registers as
 //                           the bf16 A operand and O += P.V is a wgmma with A from registers and V from smem MN-major -- V is
 //                           consumed in its natural [kv, hd] layout, no transpose.
+//
+// Schedule of a consumer warpgroup, iteration j (tile 0 issues S(0) alone, and the last P.V is issued after the loop):
+//   wait K(j), V(j-1); [turn] issue S(j) = Q.K(j)^T and O += P(j-1).V(j-1) as two wgmma groups; [hand the turn over]
+//   wait for S(j) only, release K(j); mask + softmax of tile j (the exponentials run under P(j-1).V(j-1));
+//   wait for P(j-1).V(j-1), release V(j-1); O *= alpha(j); pack P(j).
+// The two warpgroups take turns at the tensor core (named barriers 1 and 2), so one warpgroup's softmax also runs under
+// the other's MMAs.
+// Two stages suffice and cannot deadlock: the producer loads K(0), V(0), K(1), V(1), ...; iteration j needs K(j) and
+// V(j-1), and loading them needs only the releases of K(j-2) and V(j-3), made in iteration j-2 by both warpgroups.  A
+// warpgroup waiting in iteration j has taken its turn j-1, so the other one has taken at least its turn j-2 and can finish
+// iteration j-2 without waiting for anything more.
 #include <algorithm>
 #include <vector>
 
@@ -134,51 +145,59 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 
   mbar_wait(&bar_q, 0);
   const uint64_t dq = make_smem_desc_kmajor_sw128(smem_u32(smem_q) + wg * (64 * 128));
-  int st = 0;
-  uint32_t ph = 0;
-  for (int j = 0; j < n_kv; ++j) {
-    const int entry = sched[1 + j];
-    const int kt = entry >> 1;
-    const bool masked = (entry & 1) != 0;
 
-    // ---- S = Q.K^T
-    float s[64];
-    mbar_wait(&k_full[st], ph);
-    {
-      const uint64_t dk = make_smem_desc_kmajor_sw128(smem_u32(smem_k + st * ATT_TILE_BYTES));
-      wgmma_fence();
+  // S = Q.K^T of the tile in `stage`: one wgmma group.  The caller fences.
+  auto issue_qk = [&](float (&s)[64], int stage) {
+    const uint64_t dk = make_smem_desc_kmajor_sw128(smem_u32(smem_k + stage * ATT_TILE_BYTES));
 #pragma unroll
-      for (int kk = 0; kk < ATT_HD / 16; ++kk) wgmma_ss_n128(s, dq + 2 * kk, dk + 2 * kk, kk != 0 ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_reg_fence(s);
+    for (int kk = 0; kk < ATT_HD / 16; ++kk) wgmma_ss_n128(s, dq + 2 * kk, dk + 2 * kk, kk != 0 ? 1u : 0u);
+    wgmma_commit();
+  };
+  // O += P.V of the tile in `stage`: one wgmma group.  The S fragment of columns [16 kk, 16 kk + 16) is exactly the A
+  // fragment of k step kk, so P stays in registers.  The caller fences.
+  auto issue_pv = [&](const uint32_t (&pa)[ATT_BN / 16][4], int stage) {
+    const uint32_t sv = smem_u32(smem_v + stage * ATT_TILE_BYTES);
+#pragma unroll
+    for (int kk = 0; kk < ATT_BN / 16; ++kk) {
+      // V tile [128 kv x 64 hd], 128-byte rows: MN-major, 8-row k groups 1024 B apart, 16 kv rows (2048 B) per MMA
+      const uint64_t dv = make_smem_desc(sv + kk * 2048, ATT_BN * 128, 1024);
+      wgmma_rs_n64_tb(o, pa[kk], dv);
     }
-    if (lane == 0) mbar_arrive(&k_empty[st]);
-
-    if (masked) {
+    wgmma_commit();
+  };
+  // the element mask of kv tile kt on an S tile flagged partial
+  auto mask_tile = [&](float (&s)[64], int kt) {
 #pragma unroll
-      for (int i = 0; i < 16; ++i) {
+    for (int i = 0; i < 16; ++i) {
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int kv = kt * ATT_BN + 8 * i + 2 * t4 + e;
-          int sk = 0x7fffffff, tk = 0x7fffffff;   // outside the sequence: matches no row
-          if (kv < a.seq) {
-            sk = __ldg(sg + kv);
-            tk = __ldg(tm + kv);
-          }
-          if (!(sk == seg_q[0] && tk <= time_q[0])) s[4 * i + e] = -INFINITY;
-          if (!(sk == seg_q[1] && tk <= time_q[1])) s[4 * i + 2 + e] = -INFINITY;
+      for (int e = 0; e < 2; ++e) {
+        const int kv = kt * ATT_BN + 8 * i + 2 * t4 + e;
+        int sk = 0x7fffffff, tk = 0x7fffffff;   // outside the sequence: matches no row
+        if (kv < a.seq) {
+          sk = __ldg(sg + kv);
+          tk = __ldg(tm + kv);
         }
+        if (!(sk == seg_q[0] && tk <= time_q[0])) s[4 * i + e] = -INFINITY;
+        if (!(sk == seg_q[1] && tk <= time_q[1])) s[4 * i + 2 + e] = -INFINITY;
       }
     }
-
-    // ---- online softmax on the fragments: row max over the thread's columns, then over the 4 threads of the row
-    float alpha[2];
+  };
+  // online softmax of one S tile on the fragments, in place: s becomes P (fp32), m_run / l_run advance, alpha rescales O.
+  // Row max over the thread's columns as a tree (4 dependent steps after the pairs instead of 16; max is exact, so any order
+  // gives the same value), then over the 4 threads of the row.
+  auto softmax = [&](float (&s)[64], float (&alpha)[2]) {
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-      float mx = -INFINITY;
+      float m16[16];
 #pragma unroll
-      for (int i = 0; i < 16; ++i) mx = fmaxf(mx, fmaxf(s[4 * i + 2 * r], s[4 * i + 2 * r + 1]));
+      for (int i = 0; i < 16; ++i) m16[i] = fmaxf(s[4 * i + 2 * r], s[4 * i + 2 * r + 1]);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) m16[i] = fmaxf(m16[i], m16[i + 8]);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) m16[i] = fmaxf(m16[i], m16[i + 4]);
+#pragma unroll
+      for (int i = 0; i < 2; ++i) m16[i] = fmaxf(m16[i], m16[i + 2]);
+      float mx = fmaxf(m16[0], m16[1]);
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
       const float m_new = fmaxf(m_run[r], mx);
@@ -197,6 +216,19 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       }
       l_run[r] = l_run[r] * alpha[r] + sum;
     }
+  };
+  // The softmax is written out in both arms of the mask branch.  With one copy after the branch, ptxas waits for every
+  // wgmma group where the arms join, that is before the softmax, and P(j-1).V(j-1) would no longer run under it.
+  auto mask_and_softmax = [&](float (&s)[64], int entry, float (&alpha)[2]) {
+    if (entry & 1) {
+      mask_tile(s, entry >> 1);
+      softmax(s, alpha);
+    } else {
+      softmax(s, alpha);
+    }
+  };
+  // O *= alpha, then P -> the bf16 A fragments of the next P.V (all eight packed before it is issued back to back)
+  auto rescale_and_pack = [&](const float (&alpha)[2], const float (&s)[64], uint32_t (&pa)[ATT_BN / 16][4]) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       o[4 * i + 0] *= alpha[0];
@@ -204,36 +236,78 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       o[4 * i + 2] *= alpha[1];
       o[4 * i + 3] *= alpha[1];
     }
-
-    // ---- O += P.V: the S fragment of columns [16 kk, 16 kk + 16) is exactly the A fragment of k step kk
-    mbar_wait(&v_full[st], ph);
-    {
-      const uint32_t sv = smem_u32(smem_v + st * ATT_TILE_BYTES);
-      uint32_t pa[ATT_BN / 16][4];   // all eight A fragments are packed before the fence: the MMA chain is issued back to back
 #pragma unroll
-      for (int kk = 0; kk < ATT_BN / 16; ++kk) {
-        pa[kk][0] = pack_bf16x2(s[8 * kk + 0], s[8 * kk + 1]);
-        pa[kk][1] = pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]);
-        pa[kk][2] = pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]);
-        pa[kk][3] = pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7]);
-      }
+    for (int kk = 0; kk < ATT_BN / 16; ++kk) {
+      pa[kk][0] = pack_bf16x2(s[8 * kk + 0], s[8 * kk + 1]);
+      pa[kk][1] = pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]);
+      pa[kk][2] = pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]);
+      pa[kk][3] = pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7]);
+    }
+  };
+
+  // Tensor-core turns: named barrier 1 + wg is this warpgroup's turn, 2 - wg the other's (256 threads: the two consumer
+  // warpgroups).  A warpgroup issues its MMAs (S(0); S(j) and P(j-1).V(j-1); the last P.V) only in its turn and hands the
+  // turn over right after issuing, so one warpgroup's softmax runs under the other's MMAs.  Warpgroup 0 takes the first
+  // turn.  Both walk the same n_kv tiles, so both take n_kv + 1 turns, and every bar.sync meets one bar.arrive of the other
+  // warpgroup: the first turn of warpgroup 0 meets the arrive below, every later turn the arrive after the other's previous
+  // turn.  Warpgroup 1 makes no arrive after its last turn, where nothing would wait for it.  n_kv = 0 takes no turn.
+  const int my_turn = 1 + wg, other_turn = 2 - wg;
+  if (n_kv > 0) {
+    float s[64];
+    uint32_t pa[ATT_BN / 16][4];
+    float alpha[2];
+    if (wg == 1) named_bar_arrive(1, 256);
+
+    // tile 0: S(0) alone
+    mbar_wait(&k_full[0], 0);
+    named_bar_sync(my_turn, 256);
+    wgmma_fence();
+    issue_qk(s, 0);
+    named_bar_arrive(other_turn, 256);
+    wgmma_wait<0>();
+    wgmma_reg_fence(s);
+    if (lane == 0) mbar_arrive(&k_empty[0]);
+    mask_and_softmax(s, sched[1], alpha);
+    rescale_and_pack(alpha, s, pa);
+
+    // tile j: S(j) and P(j-1).V(j-1) in flight together; the softmax of tile j runs under P(j-1).V(j-1).  O is rescaled by
+    // alpha(j) after P(j-1).V(j-1) has been added, then P(j).V(j) is added in the next turn: the same operations in the same
+    // order as one tile at a time, so the same bits.
+    int st = 0;          // stage of tile j - 1
+    uint32_t ph = 0;
+    for (int j = 1; j < n_kv; ++j) {
+      const int kst = (st + 1 == ATT_STAGES) ? 0 : st + 1;
+      const uint32_t kph = (kst == 0) ? ph ^ 1 : ph;
+      mbar_wait(&k_full[kst], kph);
+      mbar_wait(&v_full[st], ph);
+      named_bar_sync(my_turn, 256);
       wgmma_reg_fence(o);
       wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < ATT_BN / 16; ++kk) {
-        // V tile [128 kv x 64 hd], 128-byte rows: MN-major, 8-row k groups 1024 B apart, 16 kv rows (2048 B) per MMA
-        const uint64_t dv = make_smem_desc(sv + kk * 2048, ATT_BN * 128, 1024);
-        wgmma_rs_n64_tb(o, pa[kk], dv);
-      }
-      wgmma_commit();
+      issue_qk(s, kst);
+      issue_pv(pa, st);
+      named_bar_arrive(other_turn, 256);
+      wgmma_wait<1>();   // S(j) has retired; P(j-1).V(j-1) may still run
+      wgmma_reg_fence(s);
+      if (lane == 0) mbar_arrive(&k_empty[kst]);
+      mask_and_softmax(s, sched[1 + j], alpha);
       wgmma_wait<0>();
       wgmma_reg_fence(o);
+      if (lane == 0) mbar_arrive(&v_empty[st]);
+      rescale_and_pack(alpha, s, pa);
+      st = kst;
+      ph = kph;
     }
+
+    // the last P.V
+    mbar_wait(&v_full[st], ph);
+    named_bar_sync(my_turn, 256);
+    wgmma_reg_fence(o);
+    wgmma_fence();
+    issue_pv(pa, st);
+    if (wg == 0) named_bar_arrive(other_turn, 256);
+    wgmma_wait<0>();
+    wgmma_reg_fence(o);
     if (lane == 0) mbar_arrive(&v_empty[st]);
-    if (++st == ATT_STAGES) {
-      st = 0;
-      ph ^= 1;
-    }
   }
 
   // ---- epilogue: O / l -> bf16 -> out[b, qpos, h*64 + ...]

@@ -201,6 +201,10 @@ __device__ __forceinline__ void setmaxnreg_dec() {
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
+// arrive on a named barrier without waiting: counts this warp's threads towards `threads`, whose bar.sync callers it releases
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 
 // D[64 x 128] (+)= A[smem, K-major] * B[smem, K-major]
 __device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
