@@ -159,7 +159,8 @@ typedef struct pf_gemm_desc {
                            * each kernel. */
   /* QKV_ROPE under sequence parallelism (peer_count > 1): head h of this rank's token chunk is stored into rank
    * (h / peer_heads)'s buffer peer_qkv[h / peer_heads], laid out [3 (q,k,v)][peer_heads][peer_seq][head_dim], at sequence
-   * position peer_row0 + (out_row_begin + m).  q_out/k_out/v_out are ignored.  batches must be 1. */
+   * position peer_row0 + (out_row_begin + m).  q_out/k_out/v_out are ignored.  batches must be 1; every peer_qkv[i] is
+   * 16-byte aligned. */
   void* peer_qkv[PF_MAX_PEERS];
   int32_t peer_count, peer_heads, peer_seq, peer_row0;
 } pf_gemm_desc;
@@ -221,7 +222,7 @@ typedef struct pf_attn_desc {
   const void* pair_mask_bits;     /* device; [blocks, 128, 4] uint32 */
   /* sequence parallelism (peer_count > 1, batch 1): row q of this rank's head group is stored into rank
    * (q / peer_chunk_rows)'s buffer peer_out[...] at row q % peer_chunk_rows, columns peer_col_begin + h*64 (row stride ldo);
-   * `out` is ignored. */
+   * `out` is ignored.  peer_col_begin % 8 == 0, peer_col_begin + heads*64 <= ldo, every peer_out[i] 16-byte aligned. */
   void* peer_out[PF_MAX_PEERS];
   int32_t peer_count, peer_chunk_rows, peer_col_begin;
   /* variant 0x20: schedule and row masks of groups of three

@@ -427,7 +427,14 @@ extern "C" int pf_attn_fwd_masked(const pf_attn_desc* d, void* stream_) {
                    static_cast<long long>(d->peer_chunk_rows) * d->peer_count >= d->seq && d->peer_col_begin % 8 == 0,
                "pf_attn_fwd_masked: bad peer layout (batch %d, count %d, chunk rows %d, seq %d)", d->batch, d->peer_count,
                d->peer_chunk_rows, d->seq);
-    for (int i = 0; i < d->peer_count; ++i) PF_REQUIRE(d->peer_out[i] != nullptr, "pf_attn_fwd_masked: peer_out[%d] is null", i);
+    // a rank's head group ends inside the row: past ldo the stores would land in the next row's columns
+    PF_REQUIRE(d->peer_col_begin >= 0 && d->peer_col_begin + static_cast<long long>(d->heads) * ATT_HD <= d->ldo,
+               "pf_attn_fwd_masked: peer columns [%d, %lld) exceed the row stride ldo %lld", d->peer_col_begin,
+               d->peer_col_begin + static_cast<long long>(d->heads) * ATT_HD, static_cast<long long>(d->ldo));
+    for (int i = 0; i < d->peer_count; ++i) {
+      PF_REQUIRE(d->peer_out[i] != nullptr, "pf_attn_fwd_masked: peer_out[%d] is null", i);
+      PF_REQUIRE((reinterpret_cast<uintptr_t>(d->peer_out[i]) & 15) == 0, "pf_attn_fwd_masked: peer_out[%d] must be 16-byte aligned", i);
+    }
   }
   if (d->lse != nullptr)
     PF_REQUIRE(d->peer_count <= 1 && d->q_row_begin == 0,

@@ -909,7 +909,11 @@ static int gemm_args_from_desc(const pf_gemm_desc* d, const char* fn, int k_alig
     PF_REQUIRE(d->peer_count <= PF_MAX_PEERS && d->peer_heads > 0 && d->peer_heads * d->peer_count >= d->heads &&
                    d->peer_row0 >= 0 && d->peer_row0 + d->out_row_begin + d->row_count <= d->peer_seq,
                "%s: bad peer layout (count %d heads/rank %d seq %d row0 %d)", fn, d->peer_count, d->peer_heads, d->peer_seq, d->peer_row0);
-    for (int i = 0; i < d->peer_count; ++i) PF_REQUIRE(d->peer_qkv[i] != nullptr, "%s: peer_qkv[%d] is null", fn, i);
+    for (int i = 0; i < d->peer_count; ++i) {
+      PF_REQUIRE(d->peer_qkv[i] != nullptr, "%s: peer_qkv[%d] is null", fn, i);
+      // the staged epilogue stores 16-byte vectors
+      PF_REQUIRE((reinterpret_cast<uintptr_t>(d->peer_qkv[i]) & 15) == 0, "%s: peer_qkv[%d] must be 16-byte aligned", fn, i);
+    }
   }
   return 0;
 }

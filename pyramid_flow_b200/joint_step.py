@@ -242,6 +242,13 @@ class JointStep(GraphedStep, torch.nn.Module):
             self._workspace(clips[-1].shape[0], plan)
 
 
+def row_ranges(text_len: int, seq: int, c0: int, c1: int):
+    """Local (row_begin, row_count) of the (text, video) parts of the token chunk [c0, c1) of the joint sequence."""
+    tb, te = max(0, c0), min(text_len, c1)
+    vb, ve = max(text_len, c0), min(seq, c1)
+    return ((tb - c0, max(0, te - tb)), (vb - c0, max(0, ve - vb)))
+
+
 class StepLaunches:
     """One call's rows, buffers and exchange arena, and the launches both models make in the same form.
 
@@ -277,16 +284,11 @@ class StepLaunches:
         if px is not None and nsp > 1:
             self.cat = px.cat(sl)
             self.qkv_x = px.qkv(s)                           # [3, Hg, S, 64]: my head group over the whole sequence
-            # the QKV epilogue stores head h of my rows into rank (h // Hg)'s gathered buffer at sequence position c0 + row;
-            # the attention epilogue stores each token chunk's rows straight into its owner's `cat`
-            self.peer_qkv = dict(peer_ptrs=[pp + px.off_qkv for pp in px.sp_buf.ptrs], peer_heads=hp // nsp, peer_seq=s,
-                                 peer_row0=c0)
-            self.peer_out = dict(peer_ptrs=[pp + px.off_cat for pp in px.sp_buf.ptrs], peer_chunk_rows=sl,
-                                 peer_col_begin=lay.sp_rank * (hp // nsp) * 64)
+            self.peer_qkv, self.peer_out = SP.peer_store_args(s, nsp, lay.sp_rank, hp,
+                                                              [pp + px.off_qkv for pp in px.sp_buf.ptrs],
+                                                              [pp + px.off_cat for pp in px.sp_buf.ptrs])
         self.rope = plan.rope[c0:c1]
-        tb, te = max(0, c0), min(t_len, c1)
-        vb, ve = max(t_len, c0), min(s, c1)
-        self.ranges = ((tb - c0, max(0, te - tb)), (vb - c0, max(0, ve - vb)))
+        self.ranges = row_ranges(t_len, s, c0, c1)
         self.seg, self.tim = plan.seg[b0:b0 + b], plan.time[b0:b0 + b]
         self.sched, self.sched2 = plan.sched[b0:b0 + b], plan.sched2[b0:b0 + b]
         self.fp8 = m.gemm_precision == "fp8"

@@ -68,6 +68,19 @@ def chunk_bounds(seq: int, sp: int, sp_rank: int) -> Tuple[int, int]:
     return sp_rank * n, (sp_rank + 1) * n
 
 
+def peer_store_args(seq: int, sp: int, sp_rank: int, hp: int, qkv_ptrs, cat_ptrs):
+    """The peer-store arguments of rank `sp_rank`'s launches (ops.gemm / ops.attn_fwd `peer=`), from the addresses of every sp
+    rank's gathered q/k/v buffer (`qkv_ptrs`, bf16 [3, hp/sp, seq, 64]) and `cat` buffer (`cat_ptrs`, rows of this rank's
+    chunk), in rank order.  The QKV epilogue stores head h of my chunk's rows into rank (h // Hg)'s gathered buffer at sequence
+    position c0 + row; the attention epilogue stores each token chunk's rows of my head group straight into its owner's `cat`,
+    at my head group's columns."""
+    c0, c1 = chunk_bounds(seq, sp, sp_rank)
+    hg = hp // sp
+    peer_qkv = dict(peer_ptrs=list(qkv_ptrs), peer_heads=hg, peer_seq=seq, peer_row0=c0)
+    peer_out = dict(peer_ptrs=list(cat_ptrs), peer_chunk_rows=c1 - c0, peer_col_begin=sp_rank * hg * 64)
+    return peer_qkv, peer_out
+
+
 def heads_to_sequence(x: torch.Tensor, lay: ParallelLayout) -> torch.Tensor:
     """Attention-boundary exchange #1 (reference B:285,295): x [Hp, S_local, hd] holds ALL (padded) heads of this rank's
     token chunk; returns [Hp/sp, S, hd] = this rank's head group over the WHOLE sequence.  One all_to_all_single."""
