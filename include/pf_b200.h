@@ -11,7 +11,7 @@
  * N = .../modeling_normalization.py, E = .../modeling_embedding.py, P = pyramid_dit/pyramid_dit_for_video_gen_pipeline.py,
  * S = diffusion_schedulers/scheduling_flow_matching.py, C = video_vae/modeling_causal_conv.py,
  * R = video_vae/modeling_resnet.py, K = video_vae/modeling_block.py, D = video_vae/modeling_enc_dec.py,
- * V = video_vae/modeling_causal_vae.py.
+ * V = video_vae/modeling_causal_vae.py, MB = pyramid_dit/mmdit_modules/modeling_mmdit_block.py.
  * The text-encoder entries cite transformers 5.5 by class and method: T5 = transformers/models/t5/modeling_t5.py,
  * CLIP = transformers/models/clip/modeling_clip.py.
  */
@@ -309,6 +309,45 @@ typedef struct pf_attn_bwd_desc {
   void* dv;
 } pf_attn_bwd_desc;
 PF_API int pf_attn_bwd_masked(const pf_attn_bwd_desc* desc, void* stream);
+
+/* ------------------------------------------------------------------ stage pack + RoPE of the training attention
+ * One stage's head-major q / k / v for pf_attn_fwd_masked / pf_attn_bwd_masked, replacing the torch glue of the training
+ * attention: the stack of q / k / v, the cat of the stage's text rows (encoder rows stage::n_stages) with its video rows, the
+ * fp32 apply_rope and transpose(1, 2) (VarlenSelfAttentionWithT5Mask B:342-360 and MB:287-305, VarlenSelfAttnSingle
+ * B:580-594; apply_rope B:34-39, MB:271-276).  Packed row s of batch b is text row s of text source row
+ * b * n_stages + stage for s < text_len, else video row row0 + s - text_len of batch b.  With freqs, q and k are rotated in
+ * fp32 without contraction and rounded once to bf16:
+ *   packed[2p + c] = fl(fl(f[b, s, p, c, 0] * x[2p]) + fl(f[b, s, p, c, 1] * x[2p + 1]));
+ * v is copied (rounded to bf16).  No accumulation, one launch.
+ *
+ * pf_attn_stage_pack_bwd is the exact inverse for gradients: it reads the packed gradients (dq, dk, dv in `packed`) and writes
+ * the stage's rows of the source gradients (the video / text pointers, in their own dtype and strides), for q and k
+ *   d x[2p + j] = fl(fl(g[2p] * f[b, s, p, 0, j]) + fl(g[2p + 1] * f[b, s, p, 1, j]))
+ * (what autograd computes through apply_rope's mul / sum_to_size / float()).  Each source row belongs to one stage, so the
+ * stages' launches together write every row of the gradients exactly once.
+ *
+ * Layout rules (checked; a violation returns <0 before any launch): head_dim 64; unit column stride; source strides in elements,
+ * positive multiples of 8, base pointers 16-byte aligned; 0 <= row0, row0 + rows <= src_rows; 0 <= stage < n_stages when
+ * text_len > 0; freqs 16-byte aligned with strides multiples of 4 and a row stride >= 128. */
+typedef struct pf_attn_pack_desc {
+  int32_t batch, heads, head_dim;
+  int32_t text_len;                /* T; 0 = no text sources (the single blocks' sequence already holds the text) */
+  int32_t rows, row0, src_rows;    /* the stage's video rows [row0, row0 + rows) of sources with src_rows rows per batch */
+  int32_t n_stages, stage;         /* text source row of batch b: b * n_stages + stage */
+  /* video sources [batch, src_rows, heads, 64] and text sources [batch * n_stages, text_len, heads, 64]: q, k, v at [0..2];
+   * strides (batch, row, head) in elements; is_f32 1 = fp32, 0 = bf16 */
+  void* video[3];
+  int64_t video_strides[3][3];
+  int32_t video_f32[3];
+  void* text[3];
+  int64_t text_strides[3][3];
+  int32_t text_f32[3];
+  const float* freqs;              /* fp32 [batch, text_len + rows, 32, 2, 2] (each row's 128 floats contiguous), or NULL */
+  int64_t freqs_batch_stride, freqs_row_stride;
+  void* packed[3];                 /* bf16 [batch, heads, text_len + rows, 64] contiguous: q, k, v (or dq, dk, dv) */
+} pf_attn_pack_desc;
+PF_API int pf_attn_stage_pack(const pf_attn_pack_desc* desc, void* stream);
+PF_API int pf_attn_stage_pack_bwd(const pf_attn_pack_desc* desc, void* stream);
 
 /* ------------------------------------------------------------------ LayerNorm + AdaLN modulate pre-pass (HBM-bound)
  * y_bf16[r, :] = LN(x_f32[r, :], eps) * (1 + scale[b, :]) + shift[b, :]   (N:174, N:234, N:120, B:1022-1023, B:1035-1036)

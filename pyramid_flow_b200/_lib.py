@@ -18,6 +18,7 @@ SYMBOLS = [
     "pf_gemm_bf16", "pf_gemm_fp8", "pf_ln_modulate_fp8", "pf_quantize_rows_fp8",
     "pf_attn_build_schedule", "pf_attn_build_pair_schedule", "pf_attn_build_pair_masks", "pf_attn_build_group_schedule",
     "pf_attn_build_group_masks", "pf_attn_fwd_masked", "pf_attn_build_kv_schedule", "pf_attn_bwd_masked",
+    "pf_attn_stage_pack", "pf_attn_stage_pack_bwd",
     "pf_ln_modulate", "pf_small_linear", "pf_timestep_embedding",
     "pf_patchify", "pf_unpatchify", "pf_cfg_euler_step", "pf_stage_hop",
     "pf_causal_conv3d", "pf_groupnorm_stats", "pf_groupnorm_apply", "pf_softmax_rows", "pf_pack_latent", "pf_blend_tiles",
@@ -80,6 +81,17 @@ class AttnBwdDesc(C.Structure):
     ]
 
 
+class AttnPackDesc(C.Structure):
+    _fields_ = [
+        ("batch", C.c_int32), ("heads", C.c_int32), ("head_dim", C.c_int32), ("text_len", C.c_int32),
+        ("rows", C.c_int32), ("row0", C.c_int32), ("src_rows", C.c_int32), ("n_stages", C.c_int32), ("stage", C.c_int32),
+        ("video", C.c_void_p * 3), ("video_strides", (C.c_int64 * 3) * 3), ("video_f32", C.c_int32 * 3),
+        ("text", C.c_void_p * 3), ("text_strides", (C.c_int64 * 3) * 3), ("text_f32", C.c_int32 * 3),
+        ("freqs", C.c_void_p), ("freqs_batch_stride", C.c_int64), ("freqs_row_stride", C.c_int64),
+        ("packed", C.c_void_p * 3),
+    ]
+
+
 class AttnTextDesc(C.Structure):
     _fields_ = [
         ("qkv", C.c_void_p), ("ld_qkv", C.c_int64), ("out", C.c_void_p), ("ldo", C.c_int64),
@@ -134,6 +146,8 @@ def load() -> C.CDLL:
                                          C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     lib.pf_attn_fwd_masked.argtypes = [C.POINTER(AttnDesc), C.c_void_p]
     lib.pf_attn_bwd_masked.argtypes = [C.POINTER(AttnBwdDesc), C.c_void_p]
+    lib.pf_attn_stage_pack.argtypes = [C.POINTER(AttnPackDesc), C.c_void_p]
+    lib.pf_attn_stage_pack_bwd.argtypes = [C.POINTER(AttnPackDesc), C.c_void_p]
     lib.pf_attn_build_kv_schedule.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     lib.pf_attn_build_schedule.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     lib.pf_attn_build_pair_schedule.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]

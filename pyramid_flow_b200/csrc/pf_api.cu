@@ -134,6 +134,46 @@ int warmup_gemm();
 int warmup_conv();
 int warmup_attn();
 int warmup_text();
+int attn_stage_pack_launch(const pf_attn_pack_desc* d, bool bwd, cudaStream_t stream);   // pf_attn_pack.cu
+
+static int check_pack_source(const char* what, const char* name, int t, const void* p, const int64_t* strides, int32_t is_f32) {
+  PF_REQUIRE(p != nullptr, "%s: %s[%d] is null", what, name, t);
+  PF_REQUIRE((reinterpret_cast<uintptr_t>(p) & 15) == 0, "%s: %s[%d] is not 16-byte aligned", what, name, t);
+  PF_REQUIRE(is_f32 == 0 || is_f32 == 1, "%s: %s_f32[%d] = %d (0 = bf16, 1 = fp32)", what, name, t, is_f32);
+  for (int i = 0; i < 3; ++i)
+    PF_REQUIRE(strides[i] > 0 && strides[i] % 8 == 0, "%s: %s[%d] stride %d = %lld, needs a positive multiple of 8 elements",
+               what, name, t, i, static_cast<long long>(strides[i]));
+  return 0;
+}
+
+// Everything the pack kernels address, checked before any launch.
+static int check_pack_desc(const pf_attn_pack_desc* d, const char* what) {
+  PF_REQUIRE(d != nullptr, "%s: null descriptor", what);
+  PF_REQUIRE(d->head_dim == 64, "%s: head_dim %d unsupported (64 only)", what, d->head_dim);
+  PF_REQUIRE(d->batch > 0 && d->batch <= 65535 && d->heads > 0 && d->rows > 0 && d->text_len >= 0,
+             "%s: bad shape (batch %d, heads %d, rows %d, text_len %d)", what, d->batch, d->heads, d->rows, d->text_len);
+  PF_REQUIRE(d->row0 >= 0 && static_cast<int64_t>(d->row0) + d->rows <= d->src_rows,
+             "%s: stage rows [%d, %lld) outside the source's %d rows", what, d->row0,
+             static_cast<long long>(d->row0) + d->rows, d->src_rows);
+  PF_REQUIRE((static_cast<int64_t>(d->text_len) + d->rows) * d->heads * 8 < (int64_t(1) << 31),
+             "%s: stage too large (%d rows x %d heads)", what, d->text_len + d->rows, d->heads);
+  for (int t = 0; t < 3; ++t) {
+    PF_REQUIRE(d->packed[t] != nullptr && (reinterpret_cast<uintptr_t>(d->packed[t]) & 15) == 0,
+               "%s: packed[%d] null or not 16-byte aligned", what, t);
+    if (int rc = check_pack_source(what, "video", t, d->video[t], d->video_strides[t], d->video_f32[t])) return rc;
+  }
+  if (d->text_len > 0) {
+    PF_REQUIRE(d->n_stages > 0 && d->stage >= 0 && d->stage < d->n_stages, "%s: stage %d of %d", what, d->stage, d->n_stages);
+    for (int t = 0; t < 3; ++t)
+      if (int rc = check_pack_source(what, "text", t, d->text[t], d->text_strides[t], d->text_f32[t])) return rc;
+  }
+  if (d->freqs != nullptr)
+    PF_REQUIRE((reinterpret_cast<uintptr_t>(d->freqs) & 15) == 0 && d->freqs_batch_stride > 0 && d->freqs_batch_stride % 4 == 0 &&
+                   d->freqs_row_stride >= 128 && d->freqs_row_stride % 4 == 0,
+               "%s: freqs must be 16-byte aligned with strides multiples of 4 and a row stride >= 128 (batch %lld, row %lld)",
+               what, static_cast<long long>(d->freqs_batch_stride), static_cast<long long>(d->freqs_row_stride));
+  return 0;
+}
 
 }  // namespace pf
 
@@ -227,6 +267,16 @@ int pf_ctx_replay(pf_ctx* c, void* stream) {
 int pf_dit_step_flux(pf_ctx* c, void* stream) { return pf_ctx_replay(c, stream); }
 int pf_dit_step_mmdit(pf_ctx* c, void* stream) { return pf_ctx_replay(c, stream); }
 int pf_vae_decode_chunk(pf_ctx* c, void* stream) { return pf_ctx_replay(c, stream); }
+
+int pf_attn_stage_pack(const pf_attn_pack_desc* d, void* stream) {
+  if (int rc = pf::check_pack_desc(d, "pf_attn_stage_pack")) return rc;
+  return pf::attn_stage_pack_launch(d, false, static_cast<cudaStream_t>(stream));
+}
+
+int pf_attn_stage_pack_bwd(const pf_attn_pack_desc* d, void* stream) {
+  if (int rc = pf::check_pack_desc(d, "pf_attn_stage_pack_bwd")) return rc;
+  return pf::attn_stage_pack_launch(d, true, static_cast<cudaStream_t>(stream));
+}
 
 int pf_set_option(int key, int value) {
   std::call_once(pf::g_options_once, pf::options_init);

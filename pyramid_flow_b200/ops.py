@@ -10,7 +10,7 @@ from typing import Optional
 import torch
 
 from . import _lib
-from ._lib import (AttnBwdDesc, AttnDesc, AttnTextDesc, GemmDesc, PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_GELU,
+from ._lib import (AttnBwdDesc, AttnDesc, AttnPackDesc, AttnTextDesc, GemmDesc, PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_GELU,
                    PF_EPI_QKV_ROPE, PF_EPI_STORE_BF16, PF_EPI_STORE_F32)
 
 
@@ -398,6 +398,63 @@ def attn_bwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tenso
     d.sched_stride = sched.shape[-1]
     d.delta, d.dq, d.dk, d.dv = delta.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr()
     _lib.check(_lib.load().pf_attn_bwd_masked(C.byref(d), _lib.stream_ptr()), "pf_attn_bwd_masked")
+
+
+def attn_pack_source_ok(t: torch.Tensor) -> bool:
+    """Whether a [B, S, H, 64] q / k / v view can be read (or, as a gradient, written) by the stage pack as it is
+    (pf_attn_stage_pack's layout rules: bf16 or fp32, unit column stride, other strides positive multiples of 8 elements,
+    16-byte aligned)."""
+    return (t.dtype in (torch.bfloat16, torch.float32) and t.ndim == 4 and t.shape[-1] == 64 and t.stride(3) == 1
+            and all(st > 0 and st % 8 == 0 for st in t.stride()[:3]) and t.data_ptr() % 16 == 0)
+
+
+def _pack_desc(video, text, freqs, packed, row0: int, stage: int, n_stages: int) -> AttnPackDesc:
+    b, h, seq, hd = packed[0].shape
+    text_len = 0 if text is None else text[0].shape[1]
+    for t in packed:
+        assert t.dtype == torch.bfloat16 and t.is_cuda and t.is_contiguous() and tuple(t.shape) == (b, h, seq, hd)
+    d = AttnPackDesc()
+    d.batch, d.heads, d.head_dim, d.text_len = b, h, hd, text_len
+    d.rows, d.row0, d.src_rows = seq - text_len, row0, video[0].shape[1]
+    d.n_stages, d.stage = n_stages, stage
+    for i, t in enumerate(video):
+        assert t.is_cuda and t.shape[0] == b and t.shape[2:] == (h, hd) and t.shape[1] == d.src_rows and attn_pack_source_ok(t), \
+            (tuple(t.shape), t.stride(), t.dtype)
+        d.video[i], d.video_f32[i] = t.data_ptr(), int(t.dtype == torch.float32)
+        for j in range(3):
+            d.video_strides[i][j] = t.stride(j)
+    if text is not None:
+        for i, t in enumerate(text):
+            assert t.is_cuda and tuple(t.shape) == (b * n_stages, text_len, h, hd) and attn_pack_source_ok(t), \
+                (tuple(t.shape), t.stride(), t.dtype)
+            d.text[i], d.text_f32[i] = t.data_ptr(), int(t.dtype == torch.float32)
+            for j in range(3):
+                d.text_strides[i][j] = t.stride(j)
+    if freqs is not None:
+        assert freqs.dtype == torch.float32 and freqs.is_cuda and freqs.numel() == b * seq * 128, tuple(freqs.shape)
+        f = freqs.reshape(b, seq, 128)
+        assert f.stride(2) == 1
+        d.freqs, d.freqs_batch_stride, d.freqs_row_stride = f.data_ptr(), f.stride(0), f.stride(1)
+    for i, t in enumerate(packed):
+        d.packed[i] = t.data_ptr()
+    return d
+
+
+def attn_stage_pack(video, text, freqs: Optional[torch.Tensor], packed, *, row0: int, stage: int = 0, n_stages: int = 1) -> None:
+    """One stage's head-major q, k, v for attn_fwd / attn_bwd (pf_attn_stage_pack): packed = (q, k, v) bf16 [B, H, T + L, 64]
+    from the text rows of encoder row b * n_stages + stage of text = (q, k, v) [B * n_stages, T, H, 64] (None: T = 0), then
+    rows [row0, row0 + L) of video = (q, k, v) [B, S_total, H, 64]; sources bf16 or fp32 views satisfying attn_pack_source_ok.
+    freqs: fp32 [B, T + L, (1,) 32, 2, 2] or None; applied to q and k as the reference's apply_rope does."""
+    d = _pack_desc(video, text, freqs, packed, row0, stage, n_stages)
+    _lib.check(_lib.load().pf_attn_stage_pack(C.byref(d), _lib.stream_ptr()), "pf_attn_stage_pack")
+
+
+def attn_stage_pack_bwd(video_grad, text_grad, freqs: Optional[torch.Tensor], packed_grad, *, row0: int, stage: int = 0,
+                        n_stages: int = 1) -> None:
+    """The gradient inverse of attn_stage_pack (pf_attn_stage_pack_bwd): reads packed_grad = (dq, dk, dv) and writes the
+    stage's rows of video_grad / text_grad (same shapes and rules as the sources, each in its own dtype)."""
+    d = _pack_desc(video_grad, text_grad, freqs, packed_grad, row0, stage, n_stages)
+    _lib.check(_lib.load().pf_attn_stage_pack_bwd(C.byref(d), _lib.stream_ptr()), "pf_attn_stage_pack_bwd")
 
 
 def attn_fwd_text(qkv: torch.Tensor, out: torch.Tensor, *, batch: int, heads: int, seq: int, scale: float,

@@ -5,12 +5,18 @@
 backward pf_attn_bwd_masked (include/pf_b200.h).  Gradients are taken w.r.t. the bf16 q / k / v with fp32 accumulation, and are
 deterministic (no atomics), so a forward recomputed under torch.utils.checkpoint gives the bits of the first one.
 
-`install_training_attention(ref_dit)` puts it under an unmodified reference `PyramidFluxTransformer` instance, trained with
-`use_flash_attn=False` (scripts/train_pyramid_flow.sh without --use_flash_attn): the `varlen_attn` callable of every
-FluxAttnProcessor2_0 / FluxSingleAttnProcessor2_0 (VarlenSelfAttentionWithT5Mask B:328-376, VarlenSelfAttnSingle B:568-606)
-is replaced by a library callable with the same signature and output layout, and the instance's `merge_input` (F:239-352)
-is wrapped so that each stage's dense [B, 1, S, S] bool mask (F:341-350) becomes a `StageAttentionPlan` carrying that stage's
+`install_training_attention(ref_dit)` puts it under an unmodified reference `PyramidFluxTransformer` or
+`PyramidDiffusionMMDiT` instance, trained with `use_flash_attn=False` (scripts/train_pyramid_flow.sh without
+--use_flash_attn): the `varlen_attn` callable of every FluxAttnProcessor2_0 / FluxSingleAttnProcessor2_0
+(VarlenSelfAttentionWithT5Mask B:328-376, VarlenSelfAttnSingle B:568-606), or the `var_len_attn` of every MMDiT
+JointAttention (VarlenSelfAttentionWithT5Mask MB:262-322, the last, context_pre_only block included), is replaced by a library
+callable with the same signature and output layout, and the instance's `merge_input` (F:239-352, M:265-380) is wrapped so
+that each stage's dense [B, 1, S, S] bool mask (F:341-350, M:369-378) becomes a `StageAttentionPlan` carrying that stage's
 seg / time ids and tile schedules.  No reference source changes; `uninstall_training_attention` restores the instance.
+
+At each call site the stacking of q / k / v, the concatenation of a stage's text rows with its video rows, the reference's
+fp32 apply_rope and the head-major transpose run as one kernel per stage (pf_attn_stage_pack), with the same bits as that
+torch code; its backward (pf_attn_stage_pack_bwd) writes the source gradients autograd would compute through it.
 """
 from __future__ import annotations
 
@@ -126,63 +132,112 @@ def _stage_plan(attention_mask, i_p: int) -> StageAttentionPlan:
     return plan
 
 
-class _JointAttention:
-    """Stands for VarlenSelfAttentionWithT5Mask (B:328-376): per stage, text tokens of that stage (encoder rows i_p::stages)
-    then its video tokens; the reference's apply_rope; attention under the stage's plan; outputs split back."""
+class _StagePack(torch.autograd.Function):
+    """Every stage of one call site packed into the kernels' head-major q / k / v (pf_attn_stage_pack, RoPE included).  The
+    forward packs all stages so that the backward (pf_attn_stage_pack_bwd per stage) writes each row of each source gradient
+    exactly once: no accumulation, and nothing of the sources is kept for the backward (only the RoPE tables)."""
 
-    def __init__(self, apply_rope):
-        self.apply_rope = apply_rope
+    @staticmethod
+    def forward(ctx, hidden_length, has_text: bool, *tensors):
+        n = len(hidden_length)
+        video = tensors[:3]
+        text = tensors[3:6] if has_text else None
+        freqs = tensors[6 if has_text else 3:] or None
+        text_len = text[0].shape[1] if text is not None else 0
+        b, _, h, hd = video[0].shape
+        packed, row0 = [], 0
+        for i_p, length in enumerate(hidden_length):
+            stage = tuple(torch.empty(b, h, text_len + length, hd, dtype=torch.bfloat16, device=video[0].device) for _ in range(3))
+            ops.attn_stage_pack(video, text, None if freqs is None else freqs[i_p], stage, row0=row0, stage=i_p, n_stages=n)
+            packed += stage
+            row0 += length
+        ctx.hidden_length, ctx.has_text = list(hidden_length), has_text
+        ctx.sources = [(t.shape, t.dtype) for t in tensors[:6 if has_text else 3]]
+        if freqs is not None:
+            ctx.save_for_backward(*freqs)
+        return tuple(packed)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        freqs = ctx.saved_tensors or None
+        dev = grads[0].device
+        dsrc = [torch.empty(shape, dtype=dt, device=dev) for shape, dt in ctx.sources]
+        dvideo, dtext = tuple(dsrc[:3]), (tuple(dsrc[3:]) if ctx.has_text else None)
+        n, row0 = len(ctx.hidden_length), 0
+        for i_p, length in enumerate(ctx.hidden_length):
+            g = tuple(t.contiguous() for t in grads[3 * i_p:3 * i_p + 3])
+            ops.attn_stage_pack_bwd(dvideo, dtext, None if freqs is None else freqs[i_p], g, row0=row0, stage=i_p, n_stages=n)
+            row0 += length
+        return (None, None, *dsrc) + (None,) * (0 if freqs is None else len(freqs))
+
+
+def _attend_stages(video, text, hidden_length, image_rotary_emb, attention_mask) -> list:
+    """The call site's attention, stage by stage: per stage i_p its text rows (encoder rows i_p::stages, when `text` is given)
+    then its video rows, the reference's apply_rope with image_rotary_emb[i_p], attention under the stage's plan.  Returns each
+    stage's output [B, T + L, H*64] in the dtype the reference's torch.stack / torch.cat of the sources gives."""
+    sources = tuple(video) + (tuple(text) if text is not None else ())
+    for t in sources:
+        if t.ndim != 4 or t.shape[-1] != HEAD_DIM:
+            raise ValueError(f"training attention: q / k / v must be [B, S, H, {HEAD_DIM}] (got {tuple(t.shape)})")
+        if t.dtype not in (torch.bfloat16, torch.float32):
+            raise ValueError(f"training attention: q / k / v must be bf16 or fp32 (got {t.dtype})")
+    b, s_total = video[0].shape[:2]
+    if sum(hidden_length) != s_total or (text is not None and text[0].shape[0] != b * len(hidden_length)):
+        raise ValueError(f"training attention: stages {list(hidden_length)} do not cover the sources "
+                         f"({tuple(video[0].shape)}{'' if text is None else f', text {tuple(text[0].shape)}'})")
+    if not video[0].is_cuda:
+        raise RuntimeError("masked_attention runs on the GPU only (pyramid_flow_b200 has no CPU path)")
+    _lib.require_device()
+    plans = [_stage_plan(attention_mask, i_p) for i_p in range(len(hidden_length))]
+    text_len = text[0].shape[1] if text is not None else 0
+    for plan, length in zip(plans, hidden_length):
+        if tuple(plan.shape) != (b, text_len + length):
+            raise ValueError(f"masked_attention: plan is for [B, S] = {tuple(plan.shape)}, the stage is {(b, text_len + length)}")
+    dt = sources[0].dtype
+    for t in sources[1:]:
+        dt = torch.promote_types(dt, t.dtype)
+    sources = tuple(t if ops.attn_pack_source_ok(t) else t.contiguous() for t in sources)
+    freqs = tuple(image_rotary_emb[i_p] for i_p in range(len(hidden_length))) if image_rotary_emb is not None else ()
+    packed = _StagePack.apply(list(hidden_length), text is not None, *sources, *freqs)
+    outs = []
+    for i_p, plan in enumerate(plans):
+        q, k, v = packed[3 * i_p:3 * i_p + 3]
+        out = _MaskedAttention.apply(q, k, v, plan, HEAD_DIM ** -0.5)
+        outs.append(out if dt == torch.bfloat16 else out.to(dt))
+    return outs
+
+
+class _JointAttention:
+    """Stands for VarlenSelfAttentionWithT5Mask (B:328-376, MB:262-322): per stage, text tokens of that stage (encoder rows
+    i_p::stages) then its video tokens; the reference's apply_rope; attention under the stage's plan; outputs split back."""
 
     def __call__(self, query, key, value, encoder_query, encoder_key, encoder_value, heads, scale, hidden_length=None,
                  image_rotary_emb=None, attention_mask=None):
         encoder_length = encoder_query.shape[1]
-        num_stages = len(hidden_length)
-        encoder_qkv = torch.stack([encoder_query, encoder_key, encoder_value], dim=2)   # [bs, sub_seq, 3, head, head_dim]
-        qkv = torch.stack([query, key, value], dim=2)
-        i_sum = 0
-        enc_out, hid_out = [], []
-        for i_p, length in enumerate(hidden_length):
-            plan = _stage_plan(attention_mask, i_p)
-            tokens = torch.cat([encoder_qkv[i_p::num_stages], qkv[:, i_sum:i_sum + length]], dim=1)
-            q, k, v = tokens.unbind(2)                                                   # [bs, tot_seq, nhead, dim]
-            if image_rotary_emb is not None:
-                q, k = self.apply_rope(q, k, image_rotary_emb[i_p])
-            out = attend(q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), plan, q.shape[-1] ** -0.5)
-            enc_out.append(out[:, :encoder_length])
-            hid_out.append(out[:, encoder_length:])
-            i_sum += length
+        outs = _attend_stages((query, key, value), (encoder_query, encoder_key, encoder_value), hidden_length,
+                              image_rotary_emb, attention_mask)
         # 'b n s d -> (b n) s d'
-        return torch.cat(hid_out, dim=1), torch.stack(enc_out, dim=1).flatten(0, 1)
+        return (torch.cat([o[:, encoder_length:] for o in outs], dim=1),
+                torch.stack([o[:, :encoder_length] for o in outs], dim=1).flatten(0, 1))
 
 
 class _SingleAttention:
     """Stands for VarlenSelfAttnSingle (B:568-606): the single blocks' joint sequence is already stage-major."""
 
-    def __init__(self, apply_rope):
-        self.apply_rope = apply_rope
-
     def __call__(self, query, key, value, heads, scale, hidden_length=None, image_rotary_emb=None, attention_mask=None):
-        qkv = torch.stack([query, key, value], dim=2)
-        i_sum = 0
-        outs = []
-        for i_p, length in enumerate(hidden_length):
-            plan = _stage_plan(attention_mask, i_p)
-            q, k, v = qkv[:, i_sum:i_sum + length].unbind(2)
-            if image_rotary_emb is not None:
-                q, k = self.apply_rope(q, k, image_rotary_emb[i_p])
-            outs.append(attend(q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), plan, q.shape[-1] ** -0.5))
-            i_sum += length
-        return torch.cat(outs, dim=1)
+        return torch.cat(_attend_stages((query, key, value), None, hidden_length, image_rotary_emb, attention_mask), dim=1)
 
 
 def stage_ids(ref_dit, sample, encoder_attention_mask: torch.Tensor, hidden_length) -> list:
-    """Per stage (seg, time) int32 [B, S_stage] of the reference's mask (F:320-350): seg 1 for valid tokens, 0 for padded
-    text (encoder_attention_mask[i_p::num_stages]); time = the temporal order ids of the model's own
-    _prepare_pyramid_image_ids, 0 for text, or 0 everywhere without use_temporal_causal."""
+    """Per stage (seg, time) int32 [B, S_stage] of the reference's mask (F:320-350, M:348-378): seg 1 for valid tokens, 0 for
+    padded text (encoder_attention_mask[i_p::num_stages]); time = the temporal order ids of the model's own
+    _prepare_pyramid_image_ids (miniFLUX) or _prepare_pyramid_temporal_rope_ids (SD3 MMDiT), 0 for text, or 0 everywhere
+    without use_temporal_causal."""
     num_stages = len(sample)
     first = sample[0][-1] if isinstance(sample[0], list) else sample[0]
     device, pad_bs = first.device, first.shape[0]
-    image_ids = ref_dit._prepare_pyramid_image_ids(sample, pad_bs, device) if ref_dit.use_temporal_causal else None
+    order_ids = getattr(ref_dit, "_prepare_pyramid_temporal_rope_ids", None) or ref_dit._prepare_pyramid_image_ids
+    image_ids = order_ids(sample, pad_bs, device) if ref_dit.use_temporal_causal else None
     out = []
     for i_p, length in enumerate(hidden_length):
         text = (encoder_attention_mask[i_p::num_stages] != 0).to(torch.int32)
@@ -199,8 +254,8 @@ def _ref_module_attr(obj, name):
 
 
 def install_training_attention(ref_dit) -> None:
-    """Run every attention of an unmodified reference PyramidFluxTransformer (use_flash_attn=False, no sequence parallelism,
-    head_dim 64) on masked_attention.  Forward values are the reference's up to bf16 rounding inside the attention; the
+    """Run every attention of an unmodified reference PyramidFluxTransformer or PyramidDiffusionMMDiT (use_flash_attn=False, no
+    sequence parallelism, head_dim 64) on masked_attention.  Forward values are the reference's up to bf16 rounding inside the attention; the
     dense masks are no longer built into the saved graph.  Idempotent; undone by uninstall_training_attention."""
     if getattr(ref_dit, "_pf_training_attention", None) is not None:
         return
@@ -218,11 +273,14 @@ def install_training_attention(ref_dit) -> None:
     for m in ref_dit.modules():
         proc = getattr(m, "processor", None)
         kind = type(proc).__name__
-        if kind not in ("FluxAttnProcessor2_0", "FluxSingleAttnProcessor2_0"):
-            continue
-        rope = _ref_module_attr(proc, "apply_rope")
-        saved.append((proc, proc.varlen_attn))
-        proc.varlen_attn = _JointAttention(rope) if kind == "FluxAttnProcessor2_0" else _SingleAttention(rope)
+        if kind in ("FluxAttnProcessor2_0", "FluxSingleAttnProcessor2_0"):           # miniFLUX: the processors' callables
+            saved.append((proc, "varlen_attn", proc.varlen_attn))
+            proc.varlen_attn = _JointAttention() if kind == "FluxAttnProcessor2_0" else _SingleAttention()
+        elif type(getattr(m, "var_len_attn", None)).__name__ == "VarlenSelfAttentionWithT5Mask":   # SD3 MMDiT: JointAttention's
+            saved.append((m, "var_len_attn", m.var_len_attn))
+            m.var_len_attn = _JointAttention()
+    if not saved:
+        raise TypeError(f"install_training_attention: no reference training attention found in {type(ref_dit).__name__}")
 
     had_own = "merge_input" in ref_dit.__dict__
     original = ref_dit.merge_input
@@ -244,8 +302,8 @@ def uninstall_training_attention(ref_dit) -> None:
     if state is None:
         return
     saved, had_own, original = state
-    for proc, fn in saved:
-        proc.varlen_attn = fn
+    for owner, name, fn in saved:
+        setattr(owner, name, fn)
     if had_own:
         ref_dit.merge_input = original
     else:

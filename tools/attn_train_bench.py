@@ -1,15 +1,19 @@
 """Training-path attention on the H100: the library's masked attention (forward + backward) against
-F.scaled_dot_product_attention with the reference's dense bool mask, and a reduced-depth reference DiT training step with and
-without install_training_attention.  One JSON line per configuration.
+F.scaled_dot_product_attention with the reference's dense bool mask; one whole call site (sources -> stage pack + RoPE ->
+attention -> output split, forward + backward) against the reference's own glue + SDPA; and a reduced-depth reference DiT
+training step with and without install_training_attention.  One JSON line per configuration.
 
-    python tools/attn_train_bench.py [--iters 10] [--warmup 3] [--skip-dit]
+    python tools/attn_train_bench.py [--iters 10] [--warmup 3] [--skip-dit] [--model flux|mmdit]
 
 Attention shape: one stage of the autoregressive 768p training run (scripts/train_pyramid_flow.sh: batch 4, temporal
 pyramid, temporal causal): 128 text tokens (T5 padding varies per sample), history frames at 1/4 and 1/2 of the 48 x 80 token
-grid (1 x 12x20 + 2 x 24x40) and the current frame at full resolution (48x80): S = 6128, 24 heads of 64.
-The DiT step: the unmodified reference PyramidFluxTransformer (staged under oracle/_ref) at miniFLUX width (24 heads) with
-2 double + 4 single blocks and gradient checkpointing, two pyramid stages of the same kind of layout, bf16 autocast; the
-two variants alternate in one process.  Times are CUDA-event medians; peak memory is torch's max_memory_allocated.
+grid (1 x 12x20 + 2 x 24x40) and the current frame at full resolution (48x80): S = 6128, 24 heads of 64.  The call site is
+that stage as a joint block sees it: bf16 q / k / v views of the Linear outputs (6000 video rows, 128 text rows), the temporal
+RoPE table, the stage's plan or dense mask built beforehand (merge_input builds them once per step for every block).
+The DiT step: the unmodified reference PyramidFluxTransformer (--model flux: miniFLUX width, 24 heads, 2 double + 4 single
+blocks) or PyramidDiffusionMMDiT (--model mmdit: SD3 width, 24 heads, 4 joint blocks, the last context_pre_only, temporal
+RoPE), staged under oracle/_ref, with gradient checkpointing, two pyramid stages of the same kind of layout, bf16 autocast.
+Paired variants alternate in one process.  Times are CUDA-event medians; peak memory is torch's max_memory_allocated.
 """
 from __future__ import annotations
 
@@ -113,15 +117,72 @@ def bench_attention(iters: int, warmup: int) -> list:
     return rows
 
 
-def bench_dit(iters: int, warmup: int) -> list:
+def _reference():
     from oracle.pin import ref_shim
     if not ref_shim.reference_available():
-        return [dict(config="dit_train_step", status="unavailable: the reference's sources are not staged (oracle/_ref)")]
+        return None
     ref_shim.install()
-    flux = __import__("pyramid_dit.flux_modules", fromlist=["PyramidFluxTransformer"]).PyramidFluxTransformer
-    model = flux(num_layers=2, num_single_layers=4, num_attention_heads=24, attention_head_dim=64, in_channels=64,
-                 joint_attention_dim=4096, pooled_projection_dim=768, use_temporal_causal=True, use_gradient_checkpointing=True,
-                 gradient_checkpointing_ratio=1.0)
+    return ref_shim
+
+
+def bench_call_site(iters: int, warmup: int) -> list:
+    ref_shim = _reference()
+    if ref_shim is None:
+        return [dict(config="call_site_fwd_bwd", status="unavailable: the reference's sources are not staged (oracle/_ref)")]
+    glue = __import__("pyramid_dit.mmdit_modules.modeling_mmdit_block",
+                      fromlist=["VarlenSelfAttentionWithT5Mask"]).VarlenSelfAttentionWithT5Mask()
+    batch, heads, text = 4, 24, 128
+    seg, time = stage_layout(batch, text, [(1, 12 * 20), (2, 24 * 40), (1, 48 * 80)])
+    s = seg.shape[1]
+    rows_video = s - text
+    g = torch.Generator(device=DEV).manual_seed(2)
+    rnd = lambda *shape: torch.randn(*shape, device=DEV, dtype=torch.bfloat16, generator=g)
+    video = [rnd(batch, rows_video, heads * 64) for _ in range(3)]        # to_q / to_k / to_v outputs
+    enc = [rnd(batch, text, heads * 64) for _ in range(3)]                 # add_q / add_k / add_v outputs (one stage)
+    ang = time.to(DEV).double()[..., None] / (10000 ** (torch.arange(0, 64, 2, device=DEV, dtype=torch.float64) / 64))
+    freqs = torch.stack([ang.cos(), -ang.sin(), ang.sin(), ang.cos()], -1).view(batch, s, 32, 2, 2).float().unsqueeze(2)
+    d_hid, d_enc = rnd(batch, rows_video, heads * 64), rnd(batch, text, heads * 64)
+    segd, timed_ = seg.to(DEV), time.to(DEV)
+    plan = training.plan_for(seg, time, DEV)
+    dense = ((segd[:, :, None] == segd[:, None, :]) & (timed_[:, :, None] >= timed_[:, None, :]))[:, None]   # M:369-378
+
+    def run(fn, mask):
+        v = [t.detach().requires_grad_() for t in video]
+        e = [t.detach().requires_grad_() for t in enc]
+        hid, enc_out = fn(*(t.view(batch, -1, heads, 64) for t in v + e), heads, 0.125, hidden_length=[rows_video],
+                          image_rotary_emb=[freqs], attention_mask=[mask])
+        torch.autograd.backward([hid, enc_out], [d_hid, d_enc])
+
+    ours = lambda: run(training._JointAttention(), plan)
+    ref = lambda: run(glue, dense)
+    rows = []
+    for name, fn in (("library_pack_kernels", ours), ("reference_glue_sdpa", ref), ("library_pack_kernels", ours),
+                     ("reference_glue_sdpa", ref)):
+        med, lo, hi = timed(fn, iters, warmup)
+        rows.append(dict(config="call_site_fwd_bwd", impl=name, batch=batch, heads=heads, seq=s, text=text,
+                         ms_median=round(med, 3), ms_min=round(lo, 3), ms_max=round(hi, 3),
+                         peak_mib=round(peak_of(fn) / 2**20, 1)))
+    return rows
+
+
+def _dit_model(ref_shim, kind: str):
+    if kind == "flux":
+        flux = __import__("pyramid_dit.flux_modules", fromlist=["PyramidFluxTransformer"]).PyramidFluxTransformer
+        return flux(num_layers=2, num_single_layers=4, num_attention_heads=24, attention_head_dim=64, in_channels=64,
+                    joint_attention_dim=4096, pooled_projection_dim=768, use_temporal_causal=True,
+                    use_gradient_checkpointing=True, gradient_checkpointing_ratio=1.0), "2+4", 768
+    mmdit = __import__("pyramid_dit.mmdit_modules", fromlist=["PyramidDiffusionMMDiT"]).PyramidDiffusionMMDiT
+    return mmdit(num_layers=4, num_attention_heads=24, attention_head_dim=64, in_channels=16, caption_projection_dim=1536,
+                 joint_attention_dim=4096, pooled_projection_dim=2048, pos_embed_type="sincos", temp_pos_embed_type="rope",
+                 add_temp_pos_embed=True, use_flash_attn=False, use_temporal_causal=True, use_gradient_checkpointing=True,
+                 gradient_checkpointing_ratio=1.0), "4 joint", 2048
+
+
+def bench_dit(iters: int, warmup: int, kind: str) -> list:
+    ref_shim = _reference()
+    if ref_shim is None:
+        return [dict(config="dit_train_step", status="unavailable: the reference's sources are not staged (oracle/_ref)")]
+    model, blocks, pooled_dim = _dit_model(ref_shim, kind)
     ref_shim.reinit_all_parameters(model, seed=0, std=0.02)
     model = model.to(DEV).train()
     bs, text = 4, 128
@@ -131,7 +192,7 @@ def bench_dit(iters: int, warmup: int) -> list:
     sample = [[rnd(bs, 16, 1, 24, 40), rnd(bs, 16, 1, 48, 80)],
               [rnd(bs, 16, 1, 24, 40), rnd(bs, 16, 2, 48, 80), rnd(bs, 16, 1, 96, 160)]]
     targets = [rnd(bs, 16, 1, 48, 80), rnd(bs, 16, 1, 96, 160)]
-    enc, pooled = rnd(2 * bs, text, 4096), rnd(2 * bs, 768)
+    enc, pooled = rnd(2 * bs, text, 4096), rnd(2 * bs, pooled_dim)
     mask = torch.ones(2 * bs, text, dtype=torch.long, device=DEV)
     for i in range(1, 2 * bs):
         mask[i, text - 9 * i:] = 0
@@ -151,7 +212,7 @@ def bench_dit(iters: int, warmup: int) -> list:
         if installed:
             training.install_training_attention(model)
         med, lo, hi = timed(step, iters, warmup)
-        rows.append(dict(config="dit_train_step", impl="installed" if installed else "reference_sdpa", blocks="2+4",
+        rows.append(dict(config="dit_train_step", model=kind, impl="installed" if installed else "reference_sdpa", blocks=blocks,
                          batch=bs, seq_per_stage=seq_per_stage,
                          ms_median=round(med, 2), ms_min=round(lo, 2), ms_max=round(hi, 2),
                          peak_mib=round(peak_of(step) / 2**20, 1)))
@@ -164,14 +225,18 @@ def main() -> None:
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--skip-dit", action="store_true")
+    ap.add_argument("--skip-call-site", action="store_true")
+    ap.add_argument("--model", choices=("flux", "mmdit"), default="flux", help="the reference DiT of the training-step leg")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("attn_train_bench: needs an H100 (no CPU measurement path)")
     _lib.require_device()
     info = device_info()
     rows = bench_attention(args.iters, args.warmup)
+    if not args.skip_call_site:
+        rows += bench_call_site(args.iters, args.warmup)
     if not args.skip_dit:
-        rows += bench_dit(args.iters, args.warmup)
+        rows += bench_dit(args.iters, args.warmup, args.model)
     for r in rows:
         print(json.dumps({**r, **info}), flush=True)
 
