@@ -349,6 +349,77 @@ typedef struct pf_attn_pack_desc {
 PF_API int pf_attn_stage_pack(const pf_attn_pack_desc* desc, void* stream);
 PF_API int pf_attn_stage_pack_bwd(const pf_attn_pack_desc* desc, void* stream);
 
+/* ------------------------------------------------------------------ varlen pack / unpack of the flash training path
+ * The padding-free form of the training attention, replacing the torch glue around flash_attn_varlen_func in
+ * VarlenFlashSelfAttentionWithT5Mask (B:189-263; called through FluxAttnProcessor2_0.varlen_flash_attn B:796-798, B:852-857)
+ * and VarlenFlashSelfAttnSingle (B:452-516; FluxSingleAttnProcessor2_0 B:736-738, B:772-777), with the per-stage
+ * `indices` / `seqlens_in_batch` of merge_input's flash branch (F:295-317).
+ *
+ * Every stage i of a call site has a padded sequence of stage_len[i] rows per batch (T + L_i: its text rows, then its video
+ * rows; the single blocks' sequence already holds the text).  A padded position p enumerates (stage, batch, row) stage-major,
+ * then batch, then row: the reference's pad_attention_mask.flatten() of each stage, concatenated.  The call site's sources
+ * for (stage i, batch b, row s) are those of pf_attn_stage_pack with stage = i, row0 = stage_row0[i]: text row s of text
+ * source row b * n_stages + i when s < text_len, else video row stage_row0[i] + s - text_len of batch b.
+ * row_map[r] is the padded position of packed row r, in the order of the reference's torch.cat(qkv_list) (each stage's
+ * `indices`, offset by the stage's first padded position); pad_map[p] is the packed row of position p, or -1 for a row the
+ * reference drops (padded text).  Both maps live on the device and are trusted: they must be inverse to each other. */
+#define PF_ATTN_VARLEN_MAX_STAGES 8
+typedef struct pf_attn_varlen_layout {
+  int32_t batch, heads, head_dim;
+  int32_t text_len;          /* T: rows of each stage's sequence held by the text sources; 0 = no text sources */
+  int32_t src_rows;          /* video source rows per batch */
+  int32_t n_stages;          /* 1 .. PF_ATTN_VARLEN_MAX_STAGES */
+  int32_t stage_len[PF_ATTN_VARLEN_MAX_STAGES];   /* rows of stage i's padded sequence per batch (> text_len) */
+  int32_t stage_row0[PF_ATTN_VARLEN_MAX_STAGES];  /* video source row of stage i's row text_len */
+  int32_t total;             /* packed rows (the sum of the cu_seqlens lengths) */
+  const int32_t* row_map;    /* device int32 [total] */
+  const int32_t* pad_map;    /* device int32 [batch * sum(stage_len)] */
+} pf_attn_varlen_layout;
+
+/* pf_attn_varlen_pack: packed row r of the head-major bf16 q / k / v [1, heads, total, 64] that pf_attn_fwd_masked /
+ * pf_attn_bwd_masked read (batch 1, seq = total) is the source row of row_map[r], with q and k rotated by stage i's table
+ * freqs[i] at (b, s) exactly as pf_attn_stage_pack does (fp32, no contraction, one rounding to bf16): the stack / cat /
+ * apply_rope (B:34-39) / index_first_axis / torch.cat of B:208-226 and B:468-483, in one launch for every stage.
+ * pf_attn_varlen_pack_bwd reads the packed gradients and writes every row of every source gradient exactly once, in the
+ * source's dtype and strides: the transposed RoPE of pf_attn_stage_pack_bwd for rows a packed row names, 0 for the others
+ * (what autograd gives through index_first_axis).  No atomics.  Sources follow the layout rules of pf_attn_stage_pack. */
+typedef struct pf_attn_varlen_pack_desc {
+  pf_attn_varlen_layout layout;
+  void* video[3];            /* [batch, src_rows, heads, 64]; strides (batch, row, head) in elements; is_f32 1 = fp32 */
+  int64_t video_strides[3][3];
+  int32_t video_f32[3];
+  void* text[3];             /* [batch * n_stages, text_len, heads, 64] (ignored when text_len = 0) */
+  int64_t text_strides[3][3];
+  int32_t text_f32[3];
+  const float* freqs[PF_ATTN_VARLEN_MAX_STAGES];  /* stage i: fp32 [batch, stage_len[i], 32, 2, 2] rows of 128 floats, or NULL */
+  int64_t freqs_batch_stride[PF_ATTN_VARLEN_MAX_STAGES], freqs_row_stride[PF_ATTN_VARLEN_MAX_STAGES];
+  void* packed[3];           /* bf16 [1, heads, total, 64] contiguous: q, k, v (or dq, dk, dv) */
+} pf_attn_varlen_pack_desc;
+PF_API int pf_attn_varlen_pack(const pf_attn_varlen_pack_desc* desc, void* stream);
+PF_API int pf_attn_varlen_pack_bwd(const pf_attn_varlen_pack_desc* desc, void* stream);
+
+/* pf_attn_varlen_unpack: the attention output [total, heads*64] (bf16, row stride ld_packed) scattered into the call site's
+ * outputs, video [batch, src_rows, heads*64] and text [batch * n_stages, text_len, heads*64], each fp32 or bf16: row s of
+ * stage i gets packed row pad_map[p], a dropped row gets 0 (pad_input into zeros_like(query) / zeros_like(encoder_query),
+ * B:201-202, B:247-258, B:464, B:504-512).  One launch; every output row written once.
+ * pf_attn_varlen_unpack_bwd gathers the output gradients (the same pointers, any strides satisfying the rules) into the
+ * packed bf16 dout [total, heads*64] that pf_attn_bwd_masked reads, rounding fp32 to bf16.
+ * Layout rules (checked): unit column stride; batch and row strides positive multiples of 8 elements, row strides >=
+ * heads*64; base pointers 16-byte aligned; ld_packed a multiple of 8, >= heads*64. */
+typedef struct pf_attn_varlen_unpack_desc {
+  pf_attn_varlen_layout layout;
+  void* video;
+  int64_t video_strides[2];  /* batch, row */
+  int32_t video_f32;
+  void* text;                /* ignored when text_len = 0 */
+  int64_t text_strides[2];
+  int32_t text_f32;
+  void* packed;
+  int64_t ld_packed;
+} pf_attn_varlen_unpack_desc;
+PF_API int pf_attn_varlen_unpack(const pf_attn_varlen_unpack_desc* desc, void* stream);
+PF_API int pf_attn_varlen_unpack_bwd(const pf_attn_varlen_unpack_desc* desc, void* stream);
+
 /* ------------------------------------------------------------------ LayerNorm + AdaLN modulate pre-pass (HBM-bound)
  * y_bf16[r, :] = LN(x_f32[r, :], eps) * (1 + scale[b, :]) + shift[b, :]   (N:174, N:234, N:120, B:1022-1023, B:1035-1036)
  * rows [row_begin, row_begin+row_count) of each batch of the joint [batches, rows_per_batch, dim] stream.

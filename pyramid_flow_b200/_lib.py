@@ -19,6 +19,7 @@ SYMBOLS = [
     "pf_attn_build_schedule", "pf_attn_build_pair_schedule", "pf_attn_build_pair_masks", "pf_attn_build_group_schedule",
     "pf_attn_build_group_masks", "pf_attn_fwd_masked", "pf_attn_build_kv_schedule", "pf_attn_bwd_masked",
     "pf_attn_stage_pack", "pf_attn_stage_pack_bwd",
+    "pf_attn_varlen_pack", "pf_attn_varlen_pack_bwd", "pf_attn_varlen_unpack", "pf_attn_varlen_unpack_bwd",
     "pf_ln_modulate", "pf_small_linear", "pf_timestep_embedding",
     "pf_patchify", "pf_unpatchify", "pf_cfg_euler_step", "pf_stage_hop",
     "pf_causal_conv3d", "pf_groupnorm_stats", "pf_groupnorm_apply", "pf_softmax_rows", "pf_pack_latent", "pf_blend_tiles",
@@ -92,6 +93,37 @@ class AttnPackDesc(C.Structure):
     ]
 
 
+VARLEN_MAX_STAGES = 8       # PF_ATTN_VARLEN_MAX_STAGES
+
+
+class AttnVarlenLayout(C.Structure):
+    _fields_ = [
+        ("batch", C.c_int32), ("heads", C.c_int32), ("head_dim", C.c_int32), ("text_len", C.c_int32), ("src_rows", C.c_int32),
+        ("n_stages", C.c_int32), ("stage_len", C.c_int32 * VARLEN_MAX_STAGES), ("stage_row0", C.c_int32 * VARLEN_MAX_STAGES),
+        ("total", C.c_int32), ("row_map", C.c_void_p), ("pad_map", C.c_void_p),
+    ]
+
+
+class AttnVarlenPackDesc(C.Structure):
+    _fields_ = [
+        ("layout", AttnVarlenLayout),
+        ("video", C.c_void_p * 3), ("video_strides", (C.c_int64 * 3) * 3), ("video_f32", C.c_int32 * 3),
+        ("text", C.c_void_p * 3), ("text_strides", (C.c_int64 * 3) * 3), ("text_f32", C.c_int32 * 3),
+        ("freqs", C.c_void_p * VARLEN_MAX_STAGES), ("freqs_batch_stride", C.c_int64 * VARLEN_MAX_STAGES),
+        ("freqs_row_stride", C.c_int64 * VARLEN_MAX_STAGES),
+        ("packed", C.c_void_p * 3),
+    ]
+
+
+class AttnVarlenUnpackDesc(C.Structure):
+    _fields_ = [
+        ("layout", AttnVarlenLayout),
+        ("video", C.c_void_p), ("video_strides", C.c_int64 * 2), ("video_f32", C.c_int32),
+        ("text", C.c_void_p), ("text_strides", C.c_int64 * 2), ("text_f32", C.c_int32),
+        ("packed", C.c_void_p), ("ld_packed", C.c_int64),
+    ]
+
+
 class AttnTextDesc(C.Structure):
     _fields_ = [
         ("qkv", C.c_void_p), ("ld_qkv", C.c_int64), ("out", C.c_void_p), ("ldo", C.c_int64),
@@ -148,6 +180,10 @@ def load() -> C.CDLL:
     lib.pf_attn_bwd_masked.argtypes = [C.POINTER(AttnBwdDesc), C.c_void_p]
     lib.pf_attn_stage_pack.argtypes = [C.POINTER(AttnPackDesc), C.c_void_p]
     lib.pf_attn_stage_pack_bwd.argtypes = [C.POINTER(AttnPackDesc), C.c_void_p]
+    for name in ("pf_attn_varlen_pack", "pf_attn_varlen_pack_bwd"):
+        getattr(lib, name).argtypes = [C.POINTER(AttnVarlenPackDesc), C.c_void_p]
+    for name in ("pf_attn_varlen_unpack", "pf_attn_varlen_unpack_bwd"):
+        getattr(lib, name).argtypes = [C.POINTER(AttnVarlenUnpackDesc), C.c_void_p]
     lib.pf_attn_build_kv_schedule.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     lib.pf_attn_build_schedule.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     lib.pf_attn_build_pair_schedule.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]

@@ -135,6 +135,8 @@ int warmup_conv();
 int warmup_attn();
 int warmup_text();
 int attn_stage_pack_launch(const pf_attn_pack_desc* d, bool bwd, cudaStream_t stream);   // pf_attn_pack.cu
+int attn_varlen_pack_launch(const pf_attn_varlen_pack_desc* d, bool bwd, cudaStream_t stream);
+int attn_varlen_unpack_launch(const pf_attn_varlen_unpack_desc* d, bool bwd, cudaStream_t stream);
 
 static int check_pack_source(const char* what, const char* name, int t, const void* p, const int64_t* strides, int32_t is_f32) {
   PF_REQUIRE(p != nullptr, "%s: %s[%d] is null", what, name, t);
@@ -172,6 +174,75 @@ static int check_pack_desc(const pf_attn_pack_desc* d, const char* what) {
                    d->freqs_row_stride >= 128 && d->freqs_row_stride % 4 == 0,
                "%s: freqs must be 16-byte aligned with strides multiples of 4 and a row stride >= 128 (batch %lld, row %lld)",
                what, static_cast<long long>(d->freqs_batch_stride), static_cast<long long>(d->freqs_row_stride));
+  return 0;
+}
+
+// The stage layout shared by the varlen pack and unpack entries (the maps' contents are the caller's, see pf_b200.h).
+static int check_varlen_layout(const pf_attn_varlen_layout& l, const char* what) {
+  PF_REQUIRE(l.head_dim == 64, "%s: head_dim %d unsupported (64 only)", what, l.head_dim);
+  PF_REQUIRE(l.batch > 0 && l.heads > 0 && l.text_len >= 0 && l.src_rows > 0 && l.total > 0,
+             "%s: bad shape (batch %d, heads %d, text_len %d, src_rows %d, total %d)", what, l.batch, l.heads, l.text_len,
+             l.src_rows, l.total);
+  PF_REQUIRE(l.n_stages >= 1 && l.n_stages <= PF_ATTN_VARLEN_MAX_STAGES, "%s: n_stages %d not in [1, %d]", what, l.n_stages,
+             PF_ATTN_VARLEN_MAX_STAGES);
+  int64_t padded = 0;
+  for (int i = 0; i < l.n_stages; ++i) {
+    PF_REQUIRE(l.stage_len[i] > l.text_len && l.stage_row0[i] >= 0 &&
+                   static_cast<int64_t>(l.stage_row0[i]) + l.stage_len[i] - l.text_len <= l.src_rows,
+               "%s: stage %d (%d rows from video row %d, text_len %d) outside the source's %d rows", what, i, l.stage_len[i],
+               l.stage_row0[i], l.text_len, l.src_rows);
+    padded += static_cast<int64_t>(l.stage_len[i]) * l.batch;
+  }
+  PF_REQUIRE(l.total <= padded, "%s: total %d exceeds the %lld padded rows", what, l.total, static_cast<long long>(padded));
+  PF_REQUIRE(padded * l.heads * 8 < (int64_t(1) << 31), "%s: too large (%lld padded rows x %d heads)", what,
+             static_cast<long long>(padded), l.heads);
+  PF_REQUIRE(l.row_map != nullptr && l.pad_map != nullptr && (reinterpret_cast<uintptr_t>(l.row_map) & 3) == 0 &&
+                 (reinterpret_cast<uintptr_t>(l.pad_map) & 3) == 0,
+             "%s: row_map / pad_map null or not 4-byte aligned", what);
+  return 0;
+}
+
+static int check_varlen_pack_desc(const pf_attn_varlen_pack_desc* d, const char* what) {
+  PF_REQUIRE(d != nullptr, "%s: null descriptor", what);
+  const pf_attn_varlen_layout& l = d->layout;
+  if (int rc = check_varlen_layout(l, what)) return rc;
+  for (int t = 0; t < 3; ++t) {
+    PF_REQUIRE(d->packed[t] != nullptr && (reinterpret_cast<uintptr_t>(d->packed[t]) & 15) == 0,
+               "%s: packed[%d] null or not 16-byte aligned", what, t);
+    if (int rc = check_pack_source(what, "video", t, d->video[t], d->video_strides[t], d->video_f32[t])) return rc;
+    if (l.text_len > 0)
+      if (int rc = check_pack_source(what, "text", t, d->text[t], d->text_strides[t], d->text_f32[t])) return rc;
+  }
+  for (int i = 0; i < l.n_stages; ++i)
+    if (d->freqs[i] != nullptr)
+      PF_REQUIRE((reinterpret_cast<uintptr_t>(d->freqs[i]) & 15) == 0 && d->freqs_batch_stride[i] > 0 &&
+                     d->freqs_batch_stride[i] % 4 == 0 && d->freqs_row_stride[i] >= 128 && d->freqs_row_stride[i] % 4 == 0,
+                 "%s: freqs[%d] must be 16-byte aligned with strides multiples of 4 and a row stride >= 128 (batch %lld, row %lld)",
+                 what, i, static_cast<long long>(d->freqs_batch_stride[i]), static_cast<long long>(d->freqs_row_stride[i]));
+  return 0;
+}
+
+static int check_unpack_rows(const char* what, const char* name, const void* p, const int64_t* strides, int32_t is_f32,
+                             int32_t heads) {
+  PF_REQUIRE(p != nullptr && (reinterpret_cast<uintptr_t>(p) & 15) == 0, "%s: %s null or not 16-byte aligned", what, name);
+  PF_REQUIRE(is_f32 == 0 || is_f32 == 1, "%s: %s_f32 = %d (0 = bf16, 1 = fp32)", what, name, is_f32);
+  PF_REQUIRE(strides[0] > 0 && strides[0] % 8 == 0 && strides[1] % 8 == 0 && strides[1] >= static_cast<int64_t>(heads) * 64,
+             "%s: %s strides (batch %lld, row %lld) need positive multiples of 8 elements and a row stride >= %d", what, name,
+             static_cast<long long>(strides[0]), static_cast<long long>(strides[1]), heads * 64);
+  return 0;
+}
+
+static int check_varlen_unpack_desc(const pf_attn_varlen_unpack_desc* d, const char* what) {
+  PF_REQUIRE(d != nullptr, "%s: null descriptor", what);
+  const pf_attn_varlen_layout& l = d->layout;
+  if (int rc = check_varlen_layout(l, what)) return rc;
+  PF_REQUIRE(d->packed != nullptr && (reinterpret_cast<uintptr_t>(d->packed) & 15) == 0 && d->ld_packed % 8 == 0 &&
+                 d->ld_packed >= static_cast<int64_t>(l.heads) * 64,
+             "%s: packed null, not 16-byte aligned, or ld_packed %lld not a multiple of 8 >= %d", what,
+             static_cast<long long>(d->ld_packed), l.heads * 64);
+  if (int rc = check_unpack_rows(what, "video", d->video, d->video_strides, d->video_f32, l.heads)) return rc;
+  if (l.text_len > 0)
+    if (int rc = check_unpack_rows(what, "text", d->text, d->text_strides, d->text_f32, l.heads)) return rc;
   return 0;
 }
 
@@ -276,6 +347,26 @@ int pf_attn_stage_pack(const pf_attn_pack_desc* d, void* stream) {
 int pf_attn_stage_pack_bwd(const pf_attn_pack_desc* d, void* stream) {
   if (int rc = pf::check_pack_desc(d, "pf_attn_stage_pack_bwd")) return rc;
   return pf::attn_stage_pack_launch(d, true, static_cast<cudaStream_t>(stream));
+}
+
+int pf_attn_varlen_pack(const pf_attn_varlen_pack_desc* d, void* stream) {
+  if (int rc = pf::check_varlen_pack_desc(d, "pf_attn_varlen_pack")) return rc;
+  return pf::attn_varlen_pack_launch(d, false, static_cast<cudaStream_t>(stream));
+}
+
+int pf_attn_varlen_pack_bwd(const pf_attn_varlen_pack_desc* d, void* stream) {
+  if (int rc = pf::check_varlen_pack_desc(d, "pf_attn_varlen_pack_bwd")) return rc;
+  return pf::attn_varlen_pack_launch(d, true, static_cast<cudaStream_t>(stream));
+}
+
+int pf_attn_varlen_unpack(const pf_attn_varlen_unpack_desc* d, void* stream) {
+  if (int rc = pf::check_varlen_unpack_desc(d, "pf_attn_varlen_unpack")) return rc;
+  return pf::attn_varlen_unpack_launch(d, false, static_cast<cudaStream_t>(stream));
+}
+
+int pf_attn_varlen_unpack_bwd(const pf_attn_varlen_unpack_desc* d, void* stream) {
+  if (int rc = pf::check_varlen_unpack_desc(d, "pf_attn_varlen_unpack_bwd")) return rc;
+  return pf::attn_varlen_unpack_launch(d, true, static_cast<cudaStream_t>(stream));
 }
 
 int pf_set_option(int key, int value) {

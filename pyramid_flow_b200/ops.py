@@ -10,7 +10,7 @@ from typing import Optional
 import torch
 
 from . import _lib
-from ._lib import (AttnBwdDesc, AttnDesc, AttnPackDesc, AttnTextDesc, GemmDesc, PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_GELU,
+from ._lib import (AttnBwdDesc, AttnDesc, AttnPackDesc, AttnTextDesc, AttnVarlenPackDesc, AttnVarlenUnpackDesc, GemmDesc, PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_GELU,
                    PF_EPI_QKV_ROPE, PF_EPI_STORE_BF16, PF_EPI_STORE_F32)
 
 
@@ -455,6 +455,88 @@ def attn_stage_pack_bwd(video_grad, text_grad, freqs: Optional[torch.Tensor], pa
     stage's rows of video_grad / text_grad (same shapes and rules as the sources, each in its own dtype)."""
     d = _pack_desc(video_grad, text_grad, freqs, packed_grad, row0, stage, n_stages)
     _lib.check(_lib.load().pf_attn_stage_pack_bwd(C.byref(d), _lib.stream_ptr()), "pf_attn_stage_pack_bwd")
+
+
+def _varlen_layout(layout, *, batch: int, heads: int, text_len: int, src_rows: int, stage_len, stage_row0, row_map, pad_map) -> None:
+    assert 1 <= len(stage_len) == len(stage_row0) <= _lib.VARLEN_MAX_STAGES, (list(stage_len), list(stage_row0))
+    for m in (row_map, pad_map):
+        assert m.dtype == torch.int32 and m.is_cuda and m.is_contiguous() and m.ndim == 1
+    assert pad_map.numel() == batch * sum(stage_len), (pad_map.numel(), batch, list(stage_len))
+    layout.batch, layout.heads, layout.head_dim, layout.text_len, layout.src_rows = batch, heads, 64, text_len, src_rows
+    layout.n_stages, layout.total = len(stage_len), row_map.numel()
+    for i, (n, r0) in enumerate(zip(stage_len, stage_row0)):
+        layout.stage_len[i], layout.stage_row0[i] = n, r0
+    layout.row_map, layout.pad_map = row_map.data_ptr(), pad_map.data_ptr()
+
+
+def attn_varlen_pack(video, text, freqs, packed, *, stage_len, stage_row0, row_map: torch.Tensor, pad_map: torch.Tensor,
+                     bwd: bool = False) -> None:
+    """Every stage of a call site packed without its dropped rows (pf_attn_varlen_pack, or with bwd=True its gradient inverse
+    pf_attn_varlen_pack_bwd): packed = (q, k, v) bf16 [1, H, total, 64]; video = (q, k, v) [B, src_rows, H, 64], text = (q, k,
+    v) [B * n_stages, T, H, 64] or None, bf16 / fp32 views satisfying attn_pack_source_ok (the gradients to write, with bwd);
+    freqs: per stage fp32 [B, stage_len[i], (1,) 32, 2, 2] or None; row_map / pad_map int32 on the device (pf_b200.h)."""
+    b, src_rows, h, hd = video[0].shape
+    total = row_map.numel()
+    text_len = 0 if text is None else text[0].shape[1]
+    d = AttnVarlenPackDesc()
+    _varlen_layout(d.layout, batch=b, heads=h, text_len=text_len, src_rows=src_rows, stage_len=stage_len, stage_row0=stage_row0,
+                   row_map=row_map, pad_map=pad_map)
+    for i, t in enumerate(packed):
+        assert t.dtype == torch.bfloat16 and t.is_cuda and t.is_contiguous() and tuple(t.shape) == (1, h, total, hd)
+        d.packed[i] = t.data_ptr()
+    for i, t in enumerate(video):
+        assert t.is_cuda and tuple(t.shape) == (b, src_rows, h, hd) and attn_pack_source_ok(t), (tuple(t.shape), t.stride(), t.dtype)
+        d.video[i], d.video_f32[i] = t.data_ptr(), int(t.dtype == torch.float32)
+        for j in range(3):
+            d.video_strides[i][j] = t.stride(j)
+    if text is not None:
+        for i, t in enumerate(text):
+            assert t.is_cuda and tuple(t.shape) == (b * len(stage_len), text_len, h, hd) and attn_pack_source_ok(t), \
+                (tuple(t.shape), t.stride(), t.dtype)
+            d.text[i], d.text_f32[i] = t.data_ptr(), int(t.dtype == torch.float32)
+            for j in range(3):
+                d.text_strides[i][j] = t.stride(j)
+    if freqs is not None:
+        for i, (f, n) in enumerate(zip(freqs, stage_len)):
+            assert f.dtype == torch.float32 and f.is_cuda and f.numel() == b * n * 128, (i, tuple(f.shape), n)
+            f = f.reshape(b, n, 128)
+            assert f.stride(2) == 1
+            d.freqs[i], d.freqs_batch_stride[i], d.freqs_row_stride[i] = f.data_ptr(), f.stride(0), f.stride(1)
+    name = "pf_attn_varlen_pack_bwd" if bwd else "pf_attn_varlen_pack"
+    _lib.check(getattr(_lib.load(), name)(C.byref(d), _lib.stream_ptr()), name)
+
+
+def attn_varlen_rows_ok(t: torch.Tensor) -> bool:
+    """Whether a [B, S, H*64] output (or output gradient) view can be written (read) by the varlen unpack as it is: bf16 or
+    fp32, unit column stride, batch and row strides positive multiples of 8 elements, 16-byte aligned."""
+    return (t.dtype in (torch.bfloat16, torch.float32) and t.ndim == 3 and t.stride(2) == 1 and t.stride(0) > 0
+            and t.stride(0) % 8 == 0 and t.stride(1) % 8 == 0 and t.stride(1) >= t.shape[2] and t.data_ptr() % 16 == 0)
+
+
+def attn_varlen_unpack(video, text, packed: torch.Tensor, *, stage_len, stage_row0, row_map: torch.Tensor, pad_map: torch.Tensor,
+                       bwd: bool = False) -> None:
+    """The attention output packed bf16 [1, total, H*64] scattered into video [B, src_rows, H*64] and text [B * n_stages, T,
+    H*64] (or None), zeros for dropped rows (pf_attn_varlen_unpack); with bwd=True the gradients video / text gathered into
+    packed (pf_attn_varlen_unpack_bwd).  video / text: bf16 or fp32 views satisfying attn_varlen_rows_ok."""
+    b, src_rows, width = video.shape
+    h = width // 64
+    assert width == h * 64 and packed.dtype == torch.bfloat16 and packed.is_cuda and packed.stride(-1) == 1
+    assert tuple(packed.shape) == (1, row_map.numel(), width), (tuple(packed.shape), row_map.numel(), width)
+    text_len = 0 if text is None else text.shape[1]
+    d = AttnVarlenUnpackDesc()
+    _varlen_layout(d.layout, batch=b, heads=h, text_len=text_len, src_rows=src_rows, stage_len=stage_len, stage_row0=stage_row0,
+                   row_map=row_map, pad_map=pad_map)
+    assert video.is_cuda and attn_varlen_rows_ok(video), (tuple(video.shape), video.stride(), video.dtype)
+    d.video, d.video_strides[0], d.video_strides[1], d.video_f32 = video.data_ptr(), video.stride(0), video.stride(1), int(
+        video.dtype == torch.float32)
+    if text is not None:
+        assert text.is_cuda and tuple(text.shape) == (b * len(stage_len), text_len, width) and attn_varlen_rows_ok(text), \
+            (tuple(text.shape), text.stride(), text.dtype)
+        d.text, d.text_strides[0], d.text_strides[1], d.text_f32 = text.data_ptr(), text.stride(0), text.stride(1), int(
+            text.dtype == torch.float32)
+    d.packed, d.ld_packed = packed.data_ptr(), packed.stride(1)
+    name = "pf_attn_varlen_unpack_bwd" if bwd else "pf_attn_varlen_unpack"
+    _lib.check(getattr(_lib.load(), name)(C.byref(d), _lib.stream_ptr()), name)
 
 
 def attn_fwd_text(qkv: torch.Tensor, out: torch.Tensor, *, batch: int, heads: int, seq: int, scale: float,

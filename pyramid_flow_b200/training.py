@@ -17,6 +17,14 @@ seg / time ids and tile schedules.  No reference source changes; `uninstall_trai
 At each call site the stacking of q / k / v, the concatenation of a stage's text rows with its video rows, the reference's
 fp32 apply_rope and the head-major transpose run as one kernel per stage (pf_attn_stage_pack), with the same bits as that
 torch code; its backward (pf_attn_stage_pack_bwd) writes the source gradients autograd would compute through it.
+
+`install_varlen_training_attention(ref_dit)` does the same for a PyramidFluxTransformer built with use_flash_attn=True
+(scripts/train_pyramid_flow_without_ar.sh): every processor's `varlen_flash_attn` (VarlenFlashSelfAttentionWithT5Mask
+B:189-263, VarlenFlashSelfAttnSingle B:452-516) is replaced, and merge_input's per-stage `indices` / `seqlens_in_batch`
+(F:295-317) become one `VarlenAttentionPlan`.  Each call site then runs three launches forward, every stage at once and without
+the padded text rows: pf_attn_varlen_pack (stack / cat / apply_rope / index_first_axis / cat), pf_attn_fwd_masked over the
+packed sequences, pf_attn_varlen_unpack (pad_input into zeros).  `varlen_attention` is the flash_attn_varlen_func subset
+the reference calls, on the same kernels.  The flash_attn package is not needed.
 """
 from __future__ import annotations
 
@@ -261,7 +269,7 @@ def install_training_attention(ref_dit) -> None:
         return
     if getattr(ref_dit, "use_flash_attn", False):
         raise ValueError("install_training_attention: the model runs the flash varlen path (use_flash_attn=True), which this "
-                         "does not replace; build it with use_flash_attn=False")
+                         "does not replace; build it with use_flash_attn=False, or use install_varlen_training_attention")
     if _ref_module_attr(ref_dit, "is_sequence_parallel_initialized")():
         raise ValueError("install_training_attention: sequence parallelism is initialised; its all-to-all attention path is "
                          "not replaced")
@@ -297,7 +305,7 @@ def install_training_attention(ref_dit) -> None:
 
 
 def uninstall_training_attention(ref_dit) -> None:
-    """Restore what install_training_attention changed on the instance."""
+    """Restore what install_training_attention or install_varlen_training_attention changed on the instance."""
     state = getattr(ref_dit, "_pf_training_attention", None)
     if state is None:
         return
@@ -309,3 +317,277 @@ def uninstall_training_attention(ref_dit) -> None:
     else:
         del ref_dit.merge_input
     del ref_dit._pf_training_attention
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# the flash varlen path: padding-free packed sequences, every stage in one attention launch
+# ----------------------------------------------------------------------------------------------------------------------
+class VarlenAttentionPlan:
+    """The packed layout of one model call's attention, for every call site: `batch` sequences per stage of stage_len[i] rows
+    (T + L_i) each; row_map int32 [total] (the padded position of each packed row, pf_b200.h pf_attn_varlen_layout) and pad_map
+    int32 [batch * sum(stage_len)] (its inverse, -1 for dropped rows); the attention mask as seg / time int32 [1, total] (seg
+    = sequence index + 1, stage-major then batch; time 0) with its tile schedules; cu_seqlens int32 [n_seq + 1] and
+    max_seqlen as flash_attn takes them.  All tensors on one device."""
+
+    def __init__(self, batch: int, stage_len, row_map, pad_map, seg, time, sched, kv_sched, cu_seqlens, max_seqlen: int):
+        self.batch, self.stage_len = batch, list(stage_len)
+        self.row_map, self.pad_map = row_map, pad_map
+        self.seg, self.time, self.sched, self.kv_sched = seg, time, sched, kv_sched
+        self.cu_seqlens, self.max_seqlen = cu_seqlens, max_seqlen
+
+    @property
+    def total(self) -> int:
+        return self.row_map.numel()
+
+    @property
+    def shape(self) -> Tuple[int, int]:
+        return tuple(self.seg.shape)
+
+
+_VARLEN_PLANS: Dict[tuple, VarlenAttentionPlan] = {}
+
+
+def varlen_plan(indices, seqlens, batch: int, stage_len, device=None) -> VarlenAttentionPlan:
+    """The VarlenAttentionPlan of merge_input's flash branch (F:295-317): per stage i the `indices` into its flattened
+    [batch, stage_len[i]] padding mask and `seqlens_in_batch` [batch].  Cached by content: one device-to-host copy per call."""
+    n = len(stage_len)
+    if not (len(indices) == len(seqlens) == n) or not 1 <= n <= _lib.VARLEN_MAX_STAGES:
+        raise ValueError(f"varlen plan: {len(indices)} indices, {len(seqlens)} seqlens for {n} stages "
+                         f"(1 .. {_lib.VARLEN_MAX_STAGES} stages)")
+    device = torch.device(device) if device is not None else indices[0].device
+    counts = [int(t.numel()) for t in indices]
+    flat = torch.cat([t.detach().reshape(-1).to(torch.int64) for t in indices] +
+                     [t.detach().reshape(-1).to(torch.int64) for t in seqlens]).cpu()       # the one device-to-host copy
+    key = (str(device), batch, tuple(stage_len), tuple(counts), flat.numpy().tobytes())
+    plan = _VARLEN_PLANS.get(key)
+    if plan is not None:
+        return plan
+    idx, lens = flat[:sum(counts)], flat[sum(counts):].view(n, -1)
+    if lens.shape[1] != batch:
+        raise ValueError(f"varlen plan: seqlens_in_batch has {lens.shape[1]} entries per stage, the batch is {batch}")
+    rows, off, pad0 = [], 0, 0
+    for i, (c, length) in enumerate(zip(counts, stage_len)):
+        ind = idx[off:off + c]
+        # the rows of (stage i, batch b) are exactly seqlens[i][b] increasing indices inside b's padded sequence
+        if c and (bool((ind[1:] <= ind[:-1]).any()) or int(ind[0]) < 0 or int(ind[-1]) >= batch * length
+                  or not torch.equal(torch.bincount(ind // length, minlength=batch), lens[i])):
+            raise ValueError(f"varlen plan: stage {i}'s indices do not match its seqlens_in_batch {lens[i].tolist()}")
+        rows.append(ind + pad0)
+        off, pad0 = off + c, pad0 + batch * length
+    if not bool((lens > 0).all()):
+        raise ValueError("varlen plan: every sequence needs at least one row")
+    plan = _make_varlen_plan(batch, stage_len, torch.cat(rows), lens.reshape(-1), device)
+    if len(_VARLEN_PLANS) >= _PLAN_CACHE_SIZE:
+        _VARLEN_PLANS.clear()
+    _VARLEN_PLANS[key] = plan
+    return plan
+
+
+def _make_varlen_plan(batch: int, stage_len, row_map: torch.Tensor, seqlens: torch.Tensor, device) -> VarlenAttentionPlan:
+    """The plan of a (CPU) row map whose packed rows hold sequences of the given lengths, one after the other."""
+    total = row_map.numel()
+    pad_map = torch.full((batch * sum(stage_len),), -1, dtype=torch.int32)
+    pad_map[row_map.long()] = torch.arange(total, dtype=torch.int32)
+    seg = torch.repeat_interleave(torch.arange(1, seqlens.numel() + 1, dtype=torch.int32), seqlens)[None]
+    time = torch.zeros_like(seg)
+    sched, _ = ops.attn_build_schedule(seg, time)
+    kv_sched = ops.attn_build_kv_schedule(sched, total)
+    cu = torch.nn.functional.pad(torch.cumsum(seqlens, 0), (1, 0)).to(torch.int32)
+    return VarlenAttentionPlan(batch, stage_len, row_map.to(device, torch.int32), pad_map.to(device), seg.to(device),
+                               time.to(device), sched.to(device), kv_sched.to(device), cu.to(device), int(seqlens.max()))
+
+
+class _VarlenPack(torch.autograd.Function):
+    """Every stage of one call site packed into head-major q / k / v [1, H, total, 64] (pf_attn_varlen_pack); the backward
+    (pf_attn_varlen_pack_bwd) writes every row of every source gradient once, 0 for the dropped rows."""
+
+    @staticmethod
+    def forward(ctx, plan: VarlenAttentionPlan, stage_row0, has_text: bool, *tensors):
+        video = tensors[:3]
+        text = tensors[3:6] if has_text else None
+        freqs = tensors[6 if has_text else 3:] or None
+        h = video[0].shape[2]
+        packed = tuple(torch.empty(1, h, plan.total, HEAD_DIM, dtype=torch.bfloat16, device=video[0].device) for _ in range(3))
+        ops.attn_varlen_pack(video, text, freqs, packed, stage_len=plan.stage_len, stage_row0=stage_row0,
+                             row_map=plan.row_map, pad_map=plan.pad_map)
+        ctx.plan, ctx.stage_row0, ctx.has_text = plan, stage_row0, has_text
+        ctx.sources = [(t.shape, t.dtype) for t in tensors[:6 if has_text else 3]]
+        if freqs is not None:
+            ctx.save_for_backward(*freqs)
+        return packed
+
+    @staticmethod
+    def backward(ctx, *grads):
+        freqs = ctx.saved_tensors or None
+        dev = grads[0].device
+        dsrc = [torch.empty(shape, dtype=dt, device=dev) for shape, dt in ctx.sources]
+        plan = ctx.plan
+        ops.attn_varlen_pack(tuple(dsrc[:3]), tuple(dsrc[3:]) if ctx.has_text else None, freqs,
+                             tuple(g.contiguous() for g in grads), stage_len=plan.stage_len, stage_row0=ctx.stage_row0,
+                             row_map=plan.row_map, pad_map=plan.pad_map, bwd=True)
+        return (None, None, None, *dsrc) + (None,) * (0 if freqs is None else len(freqs))
+
+
+class _VarlenUnpack(torch.autograd.Function):
+    """The packed attention output [1, total, H*64] scattered into the call site's outputs (pf_attn_varlen_unpack, zeros for
+    dropped rows); the backward gathers the output gradients into the packed dout (pf_attn_varlen_unpack_bwd)."""
+
+    @staticmethod
+    def forward(ctx, plan: VarlenAttentionPlan, stage_row0, out, video_shape, video_dtype, text_shape, text_dtype):
+        video = torch.empty(video_shape, dtype=video_dtype, device=out.device)
+        text = torch.empty(text_shape, dtype=text_dtype, device=out.device) if text_shape is not None else None
+        ops.attn_varlen_unpack(video, text, out, stage_len=plan.stage_len, stage_row0=stage_row0, row_map=plan.row_map,
+                               pad_map=plan.pad_map)
+        ctx.plan, ctx.stage_row0 = plan, stage_row0
+        return (video, text) if text is not None else video
+
+    @staticmethod
+    def backward(ctx, dvideo, dtext=None):
+        plan = ctx.plan
+        grads = [g if ops.attn_varlen_rows_ok(g) else g.contiguous() for g in ((dvideo, dtext) if dtext is not None else (dvideo,))]
+        dout = torch.empty(1, plan.total, grads[0].shape[-1], dtype=torch.bfloat16, device=grads[0].device)
+        ops.attn_varlen_unpack(grads[0], grads[1] if len(grads) > 1 else None, dout, stage_len=plan.stage_len,
+                               stage_row0=ctx.stage_row0, row_map=plan.row_map, pad_map=plan.pad_map, bwd=True)
+        return None, None, dout, None, None, None, None
+
+
+def _check_varlen_sources(sources) -> None:
+    for t in sources:
+        if t.ndim != 4 or t.shape[-1] != HEAD_DIM:
+            raise ValueError(f"varlen attention: q / k / v must be [B, S, H, {HEAD_DIM}] (got {tuple(t.shape)})")
+        if t.dtype not in (torch.bfloat16, torch.float32):
+            raise ValueError(f"varlen attention: q / k / v must be bf16 or fp32 (got {t.dtype})")
+    if not sources[0].is_cuda:
+        raise RuntimeError("varlen attention runs on the GPU only (pyramid_flow_b200 has no CPU path)")
+    _lib.require_device()
+
+
+def _attend_varlen(plan: VarlenAttentionPlan, video, text, stage_row0, image_rotary_emb, scale: float, out_dtypes):
+    sources = tuple(video) + (tuple(text) if text is not None else ())
+    sources = tuple(t if ops.attn_pack_source_ok(t) else t.contiguous() for t in sources)
+    freqs = tuple(image_rotary_emb[i] for i in range(len(plan.stage_len))) if image_rotary_emb is not None else ()
+    q, k, v = _VarlenPack.apply(plan, stage_row0, text is not None, *sources, *freqs)
+    out = _MaskedAttention.apply(q, k, v, plan, float(scale))
+    b, s, h, hd = video[0].shape
+    text_shape = None if text is None else (text[0].shape[0], text[0].shape[1], h * hd)
+    return _VarlenUnpack.apply(plan, stage_row0, out, (b, s, h * hd), out_dtypes[0], text_shape, out_dtypes[1])
+
+
+def _varlen_plan_arg(encoder_attention_mask) -> VarlenAttentionPlan:
+    if not isinstance(encoder_attention_mask, VarlenAttentionPlan):
+        raise TypeError("the installed varlen training attention takes the VarlenAttentionPlan of the wrapped merge_input, got "
+                        f"{type(encoder_attention_mask).__name__} (was the model's merge_input replaced after "
+                        "install_varlen_training_attention?)")
+    return encoder_attention_mask
+
+
+def _check_stages(plan: VarlenAttentionPlan, video, text_len: int, seq_lens) -> None:
+    if [text_len + n for n in seq_lens] != plan.stage_len or video[0].shape[0] != plan.batch or \
+            sum(seq_lens) != video[0].shape[1]:
+        raise ValueError(f"varlen attention: the plan is for batch {plan.batch}, stages {plan.stage_len}; the call site has "
+                         f"{tuple(video[0].shape)} with text {text_len}, stages {list(seq_lens)}")
+
+
+class _VarlenJointAttention:
+    """Stands for VarlenFlashSelfAttentionWithT5Mask (B:189-263): per stage i_p its text rows (encoder rows i_p::stages) then
+    its video rows, apply_rope with image_rotary_emb[i_p], the padded text rows dropped; one attention over every (stage,
+    batch) sequence; outputs scattered back, zeros for dropped rows."""
+
+    def __call__(self, query, key, value, encoder_query, encoder_key, encoder_value, heads, scale, hidden_length=None,
+                 image_rotary_emb=None, encoder_attention_mask=None):
+        plan = _varlen_plan_arg(encoder_attention_mask)
+        video, text = (query, key, value), (encoder_query, encoder_key, encoder_value)
+        _check_varlen_sources(video + text)
+        text_len = encoder_query.shape[1]
+        _check_stages(plan, video, text_len, hidden_length)
+        if encoder_query.shape[0] != plan.batch * len(hidden_length):
+            raise ValueError(f"varlen attention: text q / k / v {tuple(encoder_query.shape)} for batch {plan.batch} and "
+                             f"{len(hidden_length)} stages")
+        stage_row0 = [sum(hidden_length[:i]) for i in range(len(hidden_length))]
+        return _attend_varlen(plan, video, text, stage_row0, image_rotary_emb, scale, (query.dtype, encoder_query.dtype))
+
+
+class _VarlenSingleAttention:
+    """Stands for VarlenFlashSelfAttnSingle (B:452-516): the single blocks' joint sequence is already stage-major."""
+
+    def __call__(self, query, key, value, heads, scale, hidden_length=None, image_rotary_emb=None, encoder_attention_mask=None):
+        plan = _varlen_plan_arg(encoder_attention_mask)
+        video = (query, key, value)
+        _check_varlen_sources(video)
+        _check_stages(plan, video, 0, hidden_length)
+        stage_row0 = [sum(hidden_length[:i]) for i in range(len(hidden_length))]
+        return _attend_varlen(plan, video, None, stage_row0, image_rotary_emb, scale, (query.dtype, None))
+
+
+_IDENTITY_PLANS: Dict[tuple, VarlenAttentionPlan] = {}
+
+
+def varlen_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cu_seqlens: torch.Tensor,
+                     softmax_scale: Optional[float] = None) -> torch.Tensor:
+    """The subset of flash_attn_varlen_func the reference calls: non-causal self-attention within each sequence
+    [cu_seqlens[j], cu_seqlens[j + 1]), equal q and k lengths, no dropout, head_dim 64.  q, k, v token-major [total, H, 64]
+    (bf16 or fp32, rounded once to bf16); returns [total, H, 64] in q's dtype, differentiable w.r.t. q, k, v.
+    softmax_scale defaults to 64 ** -0.5."""
+    sources = tuple(t.unsqueeze(0) for t in (q, k, v))
+    if not (q.shape == k.shape == v.shape) or q.ndim != 3:
+        raise ValueError(f"varlen_attention: q, k, v must all be [total, H, {HEAD_DIM}] (got {q.shape}, {k.shape}, {v.shape})")
+    _check_varlen_sources(sources)
+    total = q.shape[0]
+    cu = cu_seqlens.detach().to("cpu", torch.int64)
+    if cu.ndim != 1 or cu.numel() < 2 or int(cu[0]) != 0 or int(cu[-1]) != total or bool((cu[1:] <= cu[:-1]).any()):
+        raise ValueError(f"varlen_attention: cu_seqlens must rise strictly from 0 to total = {total} (got {cu.tolist()})")
+    key = (str(q.device), cu.numpy().tobytes())
+    plan = _IDENTITY_PLANS.get(key)
+    if plan is None:        # one stage of one batch row holding every sequence: the identity row map
+        plan = _make_varlen_plan(1, [total], torch.arange(total), cu[1:] - cu[:-1], q.device)
+        if len(_IDENTITY_PLANS) >= _PLAN_CACHE_SIZE:
+            _IDENTITY_PLANS.clear()
+        _IDENTITY_PLANS[key] = plan
+    scale = HEAD_DIM ** -0.5 if softmax_scale is None else softmax_scale
+    out = _attend_varlen(plan, sources, None, [0], None, scale, (q.dtype, None))
+    return out.view(total, q.shape[1], HEAD_DIM)
+
+
+def install_varlen_training_attention(ref_dit) -> None:
+    """Run every attention of an unmodified reference PyramidFluxTransformer built with use_flash_attn=True (no sequence
+    parallelism, head_dim 64) on the library: the processors' varlen_flash_attn callables are replaced, merge_input's entry 6
+    (the per-stage indices / seqlens_in_batch dicts) becomes one VarlenAttentionPlan.  Forward values are the reference's up
+    to bf16 rounding inside the attention; flash_attn is not needed.  Idempotent; undone by uninstall_training_attention."""
+    if getattr(ref_dit, "_pf_training_attention", None) is not None:
+        return
+    if type(ref_dit).__name__ != "PyramidFluxTransformer":
+        raise ValueError(f"install_varlen_training_attention: {type(ref_dit).__name__} is not a miniFLUX PyramidFluxTransformer "
+                         "(the SD3 MMDiT cannot train on its flash path: it refuses use_flash_attn with use_temporal_causal)")
+    if not getattr(ref_dit, "use_flash_attn", False):
+        raise ValueError("install_varlen_training_attention: the model runs the SDPA path (use_flash_attn=False); use "
+                         "install_training_attention")
+    if _ref_module_attr(ref_dit, "is_sequence_parallel_initialized")():
+        raise ValueError("install_varlen_training_attention: sequence parallelism is initialised; its all-to-all flash path "
+                         "is not replaced")
+    head_dim = ref_dit.config.attention_head_dim
+    if head_dim != HEAD_DIM:
+        raise ValueError(f"install_varlen_training_attention: attention_head_dim {head_dim} unsupported ({HEAD_DIM} only)")
+
+    saved = []
+    for m in ref_dit.modules():
+        proc = getattr(m, "processor", None)
+        kind = type(proc).__name__
+        if kind in ("FluxAttnProcessor2_0", "FluxSingleAttnProcessor2_0"):
+            saved.append((proc, "varlen_flash_attn", proc.varlen_flash_attn))
+            proc.varlen_flash_attn = _VarlenJointAttention() if kind == "FluxAttnProcessor2_0" else _VarlenSingleAttention()
+    if not saved:
+        raise TypeError(f"install_varlen_training_attention: no flash attention processor found in {type(ref_dit).__name__}")
+
+    had_own = "merge_input" in ref_dit.__dict__
+    original = ref_dit.merge_input
+
+    def merge_input(sample, encoder_hidden_length, encoder_attention_mask):
+        res = list(original(sample, encoder_hidden_length, encoder_attention_mask))
+        stages = res[6]
+        text_len = encoder_attention_mask.shape[1]
+        res[6] = varlen_plan([st["indices"] for st in stages], [st["seqlens_in_batch"] for st in stages],
+                             int(stages[0]["seqlens_in_batch"].numel()), [text_len + n for n in res[1]])
+        return tuple(res)
+
+    ref_dit.merge_input = merge_input
+    ref_dit._pf_training_attention = (saved, had_own, original)
