@@ -495,6 +495,60 @@ typedef struct pf_conv3d_desc {
 } pf_conv3d_desc;
 PF_API int pf_causal_conv3d(const pf_conv3d_desc* desc, void* stream);
 
+/* ------------------------------------------------------------------ causal 3-D convolution backward (VAE training)
+ * Autograd of CausalConv3d.forward with temporal_chunk=False (C:116-126: F.pad(x, (1,1,1,1,2,0)) -> nn.Conv3d(padding=0),
+ * stride 1, (1,2,2) or (2,1,1)), which the reference's VAE training step (train/train_video_vae.py) runs through cuDNN.
+ *
+ * pf_conv3d_pack: src [b, c, t, h, w] (bf16 or fp32, element strides `strides`, so contiguous and channels_last_3d tensors
+ * are read in place) -> dst channels-last bf16 [b, t_total, h*dil_h, w*dil_w, cpad]; src voxel (t, h, w) lands at
+ * (t_offset + t*dil_t, h*dil_h, w*dil_w), every other element of dst (causal frames, inserted zeros, channels >= c) is
+ * written as zero.  Forward form: t_offset = kt-1, dilations 1 -- pf_causal_conv3d's x.  Gradient form: dy at t_offset 0,
+ * dilated by the conv's stride, t_total = T_in + kt - 1: the input of the data gradient (see pf_conv3d_wgrad) and the dy
+ * pf_conv3d_wgrad reads.  bias_grad (fp32 [c], or NULL): the sum of src over (b, t, h, w), from fp32 per-row partial sums
+ * added in an order fixed by the shape (workspace >= (b*t*h + min(b*t*h, 128)) * cpad floats); dy is read once for both.
+ *
+ * The data gradient has no entry of its own: it is pf_causal_conv3d at stride 1 over the dilated grid, on the packed dy
+ * (t = T_in, h = H_in, w = W_in, cin = Cout padded), with the filter flipped on all three axes and Cin / Cout swapped
+ * (wgt [Cin_pad, taps*Cout_pad], same tap-major K order), store_channels = out_c = Cin:
+ *   time: dx[s] = sum_e dy_up[s + e] W[2-e]^T;  space: dx[i] = sum_e dy_up[i + e - 1] W[2-e]^T  (dy_up = dy with zeros
+ *   inserted along a strided axis, plus kt-1 zero frames at the end because the causal padding is in front). */
+typedef struct pf_conv3d_pack_desc {
+  const void* src;
+  int32_t src_f32;
+  int32_t b, c, t, h, w;
+  int64_t strides[5]; /* element strides of src's (b, c, t, h, w) */
+  void* dst;
+  int32_t cpad, t_total, t_offset;
+  int32_t dil_t, dil_h, dil_w; /* 1 or 2 */
+  float* bias_grad;
+  float* workspace;
+  int64_t workspace_floats;
+} pf_conv3d_pack_desc;
+PF_API int pf_conv3d_pack(const pf_conv3d_pack_desc* desc, void* stream);
+/* pf_conv3d_wgrad: dw fp32 [cout_real, cin_real, kt, kh, kw] (PyTorch's Conv3d weight layout) =
+ *   sum over output voxels v of dy[v, co] * x_pad[v * stride + tap, ci]
+ * x: the forward's packed input, bf16 [b, (t-1)*stride_t + kt, h*stride_h, w*stride_w, cin]; dy: the packed gradient, bf16
+ * [b, dy_t_total, h*stride_h, w*stride_w, cout] with output voxel (t, h, w) at (t*stride_t, h*stride_h, w*stride_w) (read
+ * through TMA element strides, so the data gradient's dilated buffer serves both).  b, t, h, w are OUTPUT dims; cin / cout
+ * are the padded channel counts (multiples of 64).  The voxel range is split in a number of parts that depends on the shape
+ * only; each part's fp32 partial goes to `workspace` (pf_conv3d_wgrad_workspace floats, at most 2^26 unless one part
+ * alone is larger) and the parts are added in a fixed order: deterministic, no atomics. */
+typedef struct pf_conv3d_wgrad_desc {
+  const void* x;
+  const void* dy;
+  int32_t dy_t_total;
+  int32_t b, t, h, w;
+  int32_t cin, cout, cin_real, cout_real;
+  int32_t kt, kh, kw;
+  int32_t stride_t, stride_h, stride_w;
+  float* dw;
+  float* workspace;
+  int64_t workspace_floats;
+} pf_conv3d_wgrad_desc;
+/* floats of workspace pf_conv3d_wgrad needs for this descriptor's shape (< 0 if the descriptor is invalid) */
+PF_API int64_t pf_conv3d_wgrad_workspace(const pf_conv3d_wgrad_desc* desc);
+PF_API int pf_conv3d_wgrad(const pf_conv3d_wgrad_desc* desc, void* stream);
+
 /* per-frame GroupNorm (CausalGroupNorm C:36-43) on channels-last bf16 [frames, voxels, channels]:
  * stats[frame, group] = (mean, rstd); workspace: >= frames * 64 * channels * 2 floats.  Deterministic, and independent of
  * how many frames are passed per call (chunk-invariant).  Per-channel sums are taken in fp32 about the frame's first voxel

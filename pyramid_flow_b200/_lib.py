@@ -27,6 +27,7 @@ SYMBOLS = [
     "pf_dit_step_mmdit", "pf_vae_decode_chunk",
     "pf_peer_alloc", "pf_peer_free", "pf_peer_export", "pf_peer_open", "pf_peer_close", "pf_peer_barrier", "pf_peer_bcast",
     "pf_attn_fwd_text", "pf_rms_norm_rows", "pf_embed_tokens",
+    "pf_conv3d_pack", "pf_conv3d_wgrad_workspace", "pf_conv3d_wgrad",
 ]
 
 PF_OPT_GEMM_STAGED_RESID, PF_OPT_GEMM_WAVE_TILING, PF_OPT_ATTN_PAIR_KERNEL, PF_OPT_ATTN_TILE_PHASE, PF_OPT_ATTN_TRIPLE_KERNEL = range(5)
@@ -151,6 +152,28 @@ class ConvDesc(C.Structure):
     ]
 
 
+class ConvPackDesc(C.Structure):
+    _fields_ = [
+        ("src", C.c_void_p), ("src_f32", C.c_int32),
+        ("b", C.c_int32), ("c", C.c_int32), ("t", C.c_int32), ("h", C.c_int32), ("w", C.c_int32),
+        ("strides", C.c_int64 * 5),
+        ("dst", C.c_void_p), ("cpad", C.c_int32), ("t_total", C.c_int32), ("t_offset", C.c_int32),
+        ("dil_t", C.c_int32), ("dil_h", C.c_int32), ("dil_w", C.c_int32),
+        ("bias_grad", C.c_void_p), ("workspace", C.c_void_p), ("workspace_floats", C.c_int64),
+    ]
+
+
+class ConvWgradDesc(C.Structure):
+    _fields_ = [
+        ("x", C.c_void_p), ("dy", C.c_void_p), ("dy_t_total", C.c_int32),
+        ("b", C.c_int32), ("t", C.c_int32), ("h", C.c_int32), ("w", C.c_int32),
+        ("cin", C.c_int32), ("cout", C.c_int32), ("cin_real", C.c_int32), ("cout_real", C.c_int32),
+        ("kt", C.c_int32), ("kh", C.c_int32), ("kw", C.c_int32),
+        ("stride_t", C.c_int32), ("stride_h", C.c_int32), ("stride_w", C.c_int32),
+        ("dw", C.c_void_p), ("workspace", C.c_void_p), ("workspace_floats", C.c_int64),
+    ]
+
+
 _lib = None
 _warm_devices = set()
 
@@ -220,6 +243,10 @@ def load() -> C.CDLL:
                                  C.c_float, C.POINTER(C.c_float), C.c_void_p]
     lib.pf_blend_tiles.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_void_p]
     lib.pf_causal_conv3d.argtypes = [C.POINTER(ConvDesc), C.c_void_p]
+    lib.pf_conv3d_pack.argtypes = [C.POINTER(ConvPackDesc), C.c_void_p]
+    lib.pf_conv3d_wgrad.argtypes = [C.POINTER(ConvWgradDesc), C.c_void_p]
+    lib.pf_conv3d_wgrad_workspace.argtypes = [C.POINTER(ConvWgradDesc)]
+    lib.pf_conv3d_wgrad_workspace.restype = C.c_int64
     lib.pf_groupnorm_stats.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_float, C.c_void_p,
                                        C.c_void_p, C.c_int64, C.c_void_p]
     lib.pf_groupnorm_apply.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32,

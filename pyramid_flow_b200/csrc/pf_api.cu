@@ -132,6 +132,7 @@ int num_sms() {
 
 int warmup_gemm();
 int warmup_conv();
+int warmup_conv_bwd();
 int warmup_attn();
 int warmup_text();
 int attn_stage_pack_launch(const pf_attn_pack_desc* d, bool bwd, cudaStream_t stream);   // pf_attn_pack.cu
@@ -383,6 +384,7 @@ int pf_get_option(int key) { return pf::get_option(key); }
 int pf_warmup(void) {
   int rc = pf::warmup_gemm();
   if (!rc) rc = pf::warmup_conv();
+  if (!rc) rc = pf::warmup_conv_bwd();
   if (!rc) rc = pf::warmup_attn();
   if (!rc) rc = pf::warmup_text();
   return rc;

@@ -10,7 +10,8 @@ from typing import Optional
 import torch
 
 from . import _lib
-from ._lib import (AttnBwdDesc, AttnDesc, AttnPackDesc, AttnTextDesc, AttnVarlenPackDesc, AttnVarlenUnpackDesc, GemmDesc, PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_GELU,
+from ._lib import (AttnBwdDesc, AttnDesc, AttnPackDesc, AttnTextDesc, AttnVarlenPackDesc, AttnVarlenUnpackDesc, ConvDesc,
+                   ConvPackDesc, ConvWgradDesc, GemmDesc, PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_GELU,
                    PF_EPI_QKV_ROPE, PF_EPI_STORE_BF16, PF_EPI_STORE_F32)
 
 
@@ -584,3 +585,73 @@ def embed_tokens(ids: torch.Tensor, table: torch.Tensor, out: torch.Tensor, *, r
     _lib.check(_lib.load().pf_embed_tokens(ids.data_ptr(), ids.numel(), rows_per_batch, table.data_ptr(), table.shape[0],
                                            table.shape[1], _ptr(pos_table), max_pos, out.data_ptr(), _lib.stream_ptr()),
                "pf_embed_tokens")
+
+
+def conv3d_pack(src: torch.Tensor, dst: torch.Tensor, *, t_offset: int, dil=(1, 1, 1),
+                bias_grad: Optional[torch.Tensor] = None) -> None:
+    """src [B, C, T, H, W] (bf16 or fp32, any strides) -> dst channels-last bf16 [B, T_total, H*dil_h, W*dil_w, Cpad]
+    (pf_conv3d_pack): voxel (t, h, w) at (t_offset + t*dil_t, h*dil_h, w*dil_w), zeros elsewhere; bias_grad fp32 [C] = sum of
+    src over every axis but C."""
+    assert src.dtype in (torch.bfloat16, torch.float32) and src.dim() == 5 and src.is_cuda
+    assert dst.dtype == torch.bfloat16 and dst.is_contiguous() and dst.dim() == 5
+    b, c, t, h, w = src.shape
+    d = ConvPackDesc()
+    d.src, d.src_f32 = src.data_ptr(), int(src.dtype == torch.float32)
+    d.b, d.c, d.t, d.h, d.w = b, c, t, h, w
+    for i, s in enumerate(src.stride()):
+        d.strides[i] = s
+    d.dst, d.cpad, d.t_total, d.t_offset = dst.data_ptr(), dst.shape[-1], dst.shape[1], t_offset
+    d.dil_t, d.dil_h, d.dil_w = dil
+    assert tuple(dst.shape[2:4]) == (h * dil[1], w * dil[2]) and dst.shape[0] == b
+    ws = None
+    if bias_grad is not None:
+        assert bias_grad.dtype == torch.float32 and bias_grad.is_contiguous() and bias_grad.numel() == c
+        rows = b * t * h
+        ws = torch.empty((rows + min(rows, 128)) * dst.shape[-1], device=src.device, dtype=torch.float32)
+        d.bias_grad, d.workspace, d.workspace_floats = bias_grad.data_ptr(), ws.data_ptr(), ws.numel()
+    _lib.check(_lib.load().pf_conv3d_pack(C.byref(d), _lib.stream_ptr()), "pf_conv3d_pack")
+
+
+def causal_conv3d(x: torch.Tensor, wgt: torch.Tensor, bias: Optional[torch.Tensor], out: torch.Tensor, *, kernel, stride=(1, 1, 1),
+                  store_channels: Optional[int] = None) -> None:
+    """pf_causal_conv3d, plain store.  x bf16 [B, (t-1)*st + kt, h*sh, w*sw, cin_p] (packed, causal frames in front);
+    wgt bf16 [cout_p, taps*cin_p]; bias fp32 [cout_p] or None; out bf16 / fp32 [B, t, h, w, out_c] (the output dims)."""
+    kt, kh, kw = kernel
+    st, sh, sw = stride
+    b, t, h, w, out_c = out.shape
+    assert x.dtype == torch.bfloat16 and x.is_contiguous() and wgt.dtype == torch.bfloat16 and wgt.is_contiguous()
+    assert out.is_contiguous() and out.dtype in (torch.bfloat16, torch.float32)
+    assert tuple(x.shape[:4]) == (b, (t - 1) * st + kt, h * sh, w * sw), (tuple(x.shape), tuple(out.shape), stride)
+    assert wgt.shape[1] == kt * kh * kw * x.shape[-1]
+    assert bias is None or (bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == wgt.shape[0])
+    d = ConvDesc()
+    d.x, d.b, d.t, d.h, d.w, d.cin = x.data_ptr(), b, t, h, w, x.shape[-1]
+    d.wgt, d.bias = wgt.data_ptr(), _ptr(bias)
+    d.cout, d.kt, d.kh, d.kw = wgt.shape[0], kt, kh, kw
+    d.store_mode, d.out, d.out_f32 = 0, out.data_ptr(), int(out.dtype == torch.float32)
+    d.out_t_total, d.out_t_offset, d.out_c = t, 0, out_c
+    d.store_channels = out_c if store_channels is None else store_channels
+    d.stride_t, d.stride_h, d.stride_w = st, sh, sw
+    _lib.check(_lib.load().pf_causal_conv3d(C.byref(d), _lib.stream_ptr()), "pf_causal_conv3d")
+
+
+def conv3d_wgrad(xp: torch.Tensor, dyp: torch.Tensor, dw: torch.Tensor, *, out_shape, stride=(1, 1, 1)) -> None:
+    """dw fp32 [Cout, Cin, kt, kh, kw] (pf_conv3d_wgrad) from the packed forward input xp bf16 [B, (t-1)*st + kt, h*sh, w*sw,
+    cin_p] and the packed gradient dyp bf16 [B, T_total, h*sh, w*sw, cout_p]; out_shape = the output's (t, h, w)."""
+    t, h, w = out_shape
+    cout, cin, kt, kh, kw = dw.shape
+    assert xp.dtype == dyp.dtype == torch.bfloat16 and xp.is_contiguous() and dyp.is_contiguous()
+    assert dw.dtype == torch.float32 and dw.is_contiguous() and xp.shape[0] == dyp.shape[0]
+    d = ConvWgradDesc()
+    d.x, d.dy, d.dy_t_total = xp.data_ptr(), dyp.data_ptr(), dyp.shape[1]
+    d.b, d.t, d.h, d.w = xp.shape[0], t, h, w
+    d.cin, d.cout, d.cin_real, d.cout_real = xp.shape[-1], dyp.shape[-1], cin, cout
+    d.kt, d.kh, d.kw = kt, kh, kw
+    d.stride_t, d.stride_h, d.stride_w = stride
+    lib = _lib.load()
+    need = int(lib.pf_conv3d_wgrad_workspace(C.byref(d)))
+    if need < 0:
+        raise RuntimeError(f"libpf_b200 pf_conv3d_wgrad_workspace failed: {lib.pf_last_error().decode()}")
+    ws = torch.empty(need, device=dw.device, dtype=torch.float32)
+    d.dw, d.workspace, d.workspace_floats = dw.data_ptr(), ws.data_ptr(), need
+    _lib.check(lib.pf_conv3d_wgrad(C.byref(d), _lib.stream_ptr()), "pf_conv3d_wgrad")
