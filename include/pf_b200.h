@@ -562,6 +562,52 @@ PF_API int pf_groupnorm_stats(const void* x_bf16, int32_t frames, int64_t voxels
 PF_API int pf_groupnorm_apply(const void* x_bf16, void* y_bf16, int32_t b, int32_t t, int64_t voxels, int32_t channels,
                               int32_t groups, const float* stats, const float* gamma, const float* beta, int32_t silu,
                               int32_t y_t_total, int32_t y_t_offset, void* stream);
+/* ------------------------------------------------------------------ trainable GroupNorm (+ SiLU) (VAE training)
+ * Autograd of CausalGroupNorm.forward (C:36-43: GroupNorm of every (batch, frame) over (channels of a group) x H x W) and of
+ * the SiLU after it (CausalResnetBlock3D norm1 -> nonlinearity R:127-129, norm2 -> nonlinearity R:139-141, the encoder's /
+ * decoder's conv_norm_out -> conv_act D:194-195, D:362-363), which the reference's VAE training step runs as torch's
+ * group_norm + silu in fp32 under autocast.
+ *
+ * x: [b, c, t, h, w], bf16 or fp32, element strides x_strides, read in place in one of two forms (strides of size-1 axes
+ * are ignored): channel form, channels_last_3d (c stride 1, w stride c, h stride w*c; b and t strides multiples of 8 and
+ * x 16-byte aligned), or plane form (w stride 1, h stride w: every (b, c, t) plane contiguous, any b / c / t strides, e.g.
+ * NCDHW).  Any other layout is refused.  c % 8 == 0, c % groups == 0, c <= 2048; gamma, beta fp32 [c].
+ * pf_groupnorm_train_fwd: stats fp32 [b*t, groups, 2] = (mean, rstd) (kept for the backward);
+ *   y = act((x - mean) * rstd * gamma + beta) (act = SiLU if silu), bf16 or fp32 (y_f32), dense in x's form:
+ *   channels-last [b, t, h, w, c] for channel form, [b, c, t, h, w] for plane form.  For a bf16 channel-form x, stats and
+ *   a bf16 y are bit-identical to pf_groupnorm_stats + pf_groupnorm_apply (the same device code).
+ * pf_groupnorm_train_bwd: dy (bf16 or fp32, dy_f32) in x's form, any strides of that form; with z = xhat*gamma + beta
+ *   recomputed and dz = dy * SiLU'(z) (or dy): dbeta = sum dz, dgamma = sum dz*xhat (fp32 [c], either may be NULL) and
+ *   dx = rstd * (gamma dz - mean(gamma dz) - xhat mean(gamma dz xhat)) (means per frame and group) in x's dtype, dense in
+ *   x's form (NULL: not computed).  x and dy are read twice (once for dx), dx written once.
+ * Both need a workspace of pf_groupnorm_train_workspace floats (per (frame, split, channel) fp32 partial sums); the split
+ * count depends on h*w only, there are no atomics: the bits depend on the shape alone. */
+typedef struct pf_groupnorm_train_desc {
+  const void* x;
+  int32_t x_f32;
+  int32_t b, c, t, h, w;
+  int64_t x_strides[5]; /* element strides of x's (b, c, t, h, w) */
+  int32_t groups;
+  float eps;
+  int32_t silu;
+  const float* gamma;
+  const float* beta;
+  float* stats;         /* [b*t, groups, 2]: written by the forward, read by the backward */
+  void* y;              /* forward output */
+  int32_t y_f32;
+  const void* dy;       /* backward input */
+  int32_t dy_f32;
+  int64_t dy_strides[5];
+  void* dx;             /* backward outputs */
+  float* dgamma;
+  float* dbeta;
+  float* workspace;
+  int64_t workspace_floats;
+} pf_groupnorm_train_desc;
+/* floats of workspace the forward and the backward need for this descriptor's shape (< 0 if the descriptor is invalid) */
+PF_API int64_t pf_groupnorm_train_workspace(const pf_groupnorm_train_desc* desc);
+PF_API int pf_groupnorm_train_fwd(const pf_groupnorm_train_desc* desc, void* stream);
+PF_API int pf_groupnorm_train_bwd(const pf_groupnorm_train_desc* desc, void* stream);
 /* in-place row softmax of bf16 scores [rows, ld]: softmax over the first `cols` columns of scale*s, zeros in the padding
  * (mid-block attention, diffusers Attention used at K:454-460). */
 PF_API int pf_softmax_rows(void* s_bf16, int64_t rows, int32_t cols, int64_t ld, float scale, void* stream);

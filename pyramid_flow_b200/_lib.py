@@ -28,6 +28,7 @@ SYMBOLS = [
     "pf_peer_alloc", "pf_peer_free", "pf_peer_export", "pf_peer_open", "pf_peer_close", "pf_peer_barrier", "pf_peer_bcast",
     "pf_attn_fwd_text", "pf_rms_norm_rows", "pf_embed_tokens",
     "pf_conv3d_pack", "pf_conv3d_wgrad_workspace", "pf_conv3d_wgrad",
+    "pf_groupnorm_train_workspace", "pf_groupnorm_train_fwd", "pf_groupnorm_train_bwd",
 ]
 
 PF_OPT_GEMM_STAGED_RESID, PF_OPT_GEMM_WAVE_TILING, PF_OPT_ATTN_PAIR_KERNEL, PF_OPT_ATTN_TILE_PHASE, PF_OPT_ATTN_TRIPLE_KERNEL = range(5)
@@ -174,6 +175,20 @@ class ConvWgradDesc(C.Structure):
     ]
 
 
+class GroupNormTrainDesc(C.Structure):
+    _fields_ = [
+        ("x", C.c_void_p), ("x_f32", C.c_int32),
+        ("b", C.c_int32), ("c", C.c_int32), ("t", C.c_int32), ("h", C.c_int32), ("w", C.c_int32),
+        ("x_strides", C.c_int64 * 5),
+        ("groups", C.c_int32), ("eps", C.c_float), ("silu", C.c_int32),
+        ("gamma", C.c_void_p), ("beta", C.c_void_p), ("stats", C.c_void_p),
+        ("y", C.c_void_p), ("y_f32", C.c_int32),
+        ("dy", C.c_void_p), ("dy_f32", C.c_int32), ("dy_strides", C.c_int64 * 5),
+        ("dx", C.c_void_p), ("dgamma", C.c_void_p), ("dbeta", C.c_void_p),
+        ("workspace", C.c_void_p), ("workspace_floats", C.c_int64),
+    ]
+
+
 _lib = None
 _warm_devices = set()
 
@@ -247,6 +262,10 @@ def load() -> C.CDLL:
     lib.pf_conv3d_wgrad.argtypes = [C.POINTER(ConvWgradDesc), C.c_void_p]
     lib.pf_conv3d_wgrad_workspace.argtypes = [C.POINTER(ConvWgradDesc)]
     lib.pf_conv3d_wgrad_workspace.restype = C.c_int64
+    for name in ("pf_groupnorm_train_fwd", "pf_groupnorm_train_bwd"):
+        getattr(lib, name).argtypes = [C.POINTER(GroupNormTrainDesc), C.c_void_p]
+    lib.pf_groupnorm_train_workspace.argtypes = [C.POINTER(GroupNormTrainDesc)]
+    lib.pf_groupnorm_train_workspace.restype = C.c_int64
     lib.pf_groupnorm_stats.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_float, C.c_void_p,
                                        C.c_void_p, C.c_int64, C.c_void_p]
     lib.pf_groupnorm_apply.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32,

@@ -2,101 +2,31 @@
 //   per-frame GroupNorm statistics + apply(+SiLU) (CausalGroupNorm C:36-43, R:127-141, D:362-363),
 //   row softmax for the mid-block attention (diffusers Attention, K:454-460), latent layout packing.
 #include "../../include/pf_b200.h"
-#include "pf_common.cuh"
+#include "pf_groupnorm.cuh"
 
 namespace pf {
 
-// ---------------------------------------------------------------------------------------------------------------
-// GroupNorm statistics, pass 1: per (frame, split) partial sum / sum-of-squares per CHANNEL of x - K, with the pivot
-// K = x[frame, voxel 0, channel].  Unshifted fp32 sums lose the variance to cancellation in E[x^2] - mean^2 once a
-// group's |mean| is large against its std (~4% rstd error at |mean|/std = 100); shifted by a value inside the channel's
-// own distribution they stay accurate.  Every thread reads the same pivot, so the sums remain deterministic and
-// independent of how frames are split across calls.
-// Each thread owns one 8-channel vector position and strides over voxels; 128-bit loads, fp32 partials.
-// ---------------------------------------------------------------------------------------------------------------
+// GroupNorm statistics on channels-last bf16 frames [frames, voxels, channels]: pass 1 writes per (frame, split) partial
+// sums per channel (gn_partial_frame, pf_groupnorm.cuh), pass 2 combines them per (frame, group) in double.  The training
+// GroupNorm (pf_groupnorm_train.cu) runs the same device code.
 __global__ void __launch_bounds__(256)
 gn_partial_kernel(const __nv_bfloat16* __restrict__ x, long long voxels, int channels, int nsplit,
                   float* __restrict__ partial /* [frames, nsplit, channels, 2] */) {
-  // deterministic: per-thread partials are parked in shared memory [vstep][channels][2] and summed in a fixed order
   extern __shared__ float sh[];
   const int frame = blockIdx.x / nsplit;
   const int split = blockIdx.x - frame * nsplit;
-  const int cvecs = channels >> 3;
-  const long long v0 = voxels * split / nsplit, v1 = voxels * (split + 1) / nsplit;
-  const int cv = threadIdx.x % cvecs;
-  const int vlane = threadIdx.x / cvecs;
-  const int vstep = blockDim.x / cvecs;
-  float s[8], ss[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) s[i] = ss[i] = 0.f;
-  if (vlane < vstep) {
-    const __nv_bfloat16* base = x + static_cast<size_t>(frame) * voxels * channels;
-    float k[8];
-    {
-      const uint4 u = __ldg(reinterpret_cast<const uint4*>(base) + cv);
-      const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = __bfloat1622float2(h[i]);
-        k[2 * i] = f.x;
-        k[2 * i + 1] = f.y;
-      }
-    }
-    for (long long v = v0 + vlane; v < v1; v += vstep) {
-      const uint4 u = __ldg(reinterpret_cast<const uint4*>(base + v * channels) + cv);
-      const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = __bfloat1622float2(h[i]);
-        const float d0 = f.x - k[2 * i], d1 = f.y - k[2 * i + 1];   // exact for bf16 operands within 2^16 of each other
-        s[2 * i] += d0; ss[2 * i] += d0 * d0;
-        s[2 * i + 1] += d1; ss[2 * i + 1] += d1 * d1;
-      }
-    }
-    float* dst = sh + (static_cast<size_t>(vlane) * channels + cv * 8) * 2;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      dst[2 * i] = s[i];
-      dst[2 * i + 1] = ss[i];
-    }
-  }
-  __syncthreads();
-  float* out = partial + (static_cast<size_t>(frame) * nsplit + split) * channels * 2;
-  for (int i = threadIdx.x; i < 2 * channels; i += blockDim.x) {
-    float acc = 0.f;
-    for (int l = 0; l < vstep; ++l) acc += sh[static_cast<size_t>(l) * channels * 2 + i];
-    out[i] = acc;
-  }
+  gn_partial_frame(x + static_cast<size_t>(frame) * voxels * channels, channels, voxels * split / nsplit,
+                   voxels * (split + 1) / nsplit, partial + (static_cast<size_t>(frame) * nsplit + split) * channels * 2, sh);
 }
 
-// pass 2: (mean, rstd) per (frame, group), combined in double: per channel the shifted sums S = sum(x - K) and
-// SS = sum((x - K)^2) give sum(x) = S + nK and sum(x^2) = SS + 2KS + nK^2
 __global__ void gn_finalize_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ partial, int frames,
                                    int nsplit, int channels, int groups, long long voxels, float eps,
                                    float* __restrict__ stats /* [frames, groups, 2] */) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= frames * groups) return;
   const int frame = idx / groups, g = idx - frame * groups;
-  const int cpg = channels / groups;
-  const double nv = static_cast<double>(voxels);
-  double s = 0.0, ss = 0.0;
-  for (int c = g * cpg; c < (g + 1) * cpg; ++c) {
-    double sc = 0.0, ssc = 0.0;
-    for (int sp = 0; sp < nsplit; ++sp) {
-      const float* p = partial + ((static_cast<size_t>(frame) * nsplit + sp) * channels + c) * 2;
-      sc += p[0];
-      ssc += p[1];
-    }
-    const double k = __bfloat162float(x[static_cast<size_t>(frame) * voxels * channels + c]);
-    s += sc + nv * k;
-    ss += ssc + 2.0 * k * sc + nv * k * k;
-  }
-  const double n = nv * cpg;
-  const double mean = s / n;
-  double var = ss / n - mean * mean;
-  if (var < 0.0) var = 0.0;
-  stats[2 * idx] = static_cast<float>(mean);
-  stats[2 * idx + 1] = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
+  gn_finalize_group(x + static_cast<size_t>(frame) * voxels * channels, 1, partial + static_cast<size_t>(frame) * nsplit * channels * 2,
+                    nsplit, channels, g, channels / groups, voxels, eps, stats + 2 * idx);
 }
 
 // apply: y[b, t + t_off, vox, c] = act((x[b, t, vox, c] - mean) * rstd * gamma[c] + beta[c]); 8 channels per thread
@@ -131,9 +61,7 @@ gn_apply_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__
     const int g = c / cpg;
     const float mean = __ldg(stats + 2 * (frame * groups + g));
     const float rstd = __ldg(stats + 2 * (frame * groups + g) + 1);
-    float v = (o[i] - mean) * rstd * __ldg(gamma + c) + __ldg(beta + c);
-    if (silu) v = silu_f(v);
-    o[i] = v;
+    o[i] = gn_affine_act(o[i], mean, rstd, __ldg(gamma + c), __ldg(beta + c), silu);
   }
   uint4 w;
   w.x = pack_bf16x2(o[0], o[1]);
@@ -218,9 +146,7 @@ int pf_groupnorm_stats(const void* x, int32_t frames, int64_t voxels, int32_t ch
   PF_REQUIRE(channels % 8 == 0 && channels % groups == 0 && channels <= 2048, "pf_groupnorm_stats: channels=%d unsupported", channels);
   // the split count depends on the frame SIZE only, never on how many frames are in the call: per-frame statistics are
   // bitwise identical whatever the temporal chunking
-  long long nsplit = (voxels + 4095) / 4096;
-  if (nsplit < 1) nsplit = 1;
-  if (nsplit > 64) nsplit = 64;
+  const long long nsplit = gn_splits(voxels);
   PF_REQUIRE(static_cast<long long>(frames) * nsplit * channels * 2 <= workspace_floats, "pf_groupnorm_stats: workspace too small (need %lld floats)",
              static_cast<long long>(frames) * nsplit * channels * 2);
   const int vstep = 256 / (channels / 8);

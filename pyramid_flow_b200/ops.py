@@ -11,7 +11,7 @@ import torch
 
 from . import _lib
 from ._lib import (AttnBwdDesc, AttnDesc, AttnPackDesc, AttnTextDesc, AttnVarlenPackDesc, AttnVarlenUnpackDesc, ConvDesc,
-                   ConvPackDesc, ConvWgradDesc, GemmDesc, PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_GELU,
+                   ConvPackDesc, ConvWgradDesc, GemmDesc, GroupNormTrainDesc, PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_GELU,
                    PF_EPI_QKV_ROPE, PF_EPI_STORE_BF16, PF_EPI_STORE_F32)
 
 
@@ -655,3 +655,80 @@ def conv3d_wgrad(xp: torch.Tensor, dyp: torch.Tensor, dw: torch.Tensor, *, out_s
     ws = torch.empty(need, device=dw.device, dtype=torch.float32)
     d.dw, d.workspace, d.workspace_floats = dw.data_ptr(), ws.data_ptr(), need
     _lib.check(lib.pf_conv3d_wgrad(C.byref(d), _lib.stream_ptr()), "pf_conv3d_wgrad")
+
+
+def groupnorm_form(x: torch.Tensor) -> Optional[str]:
+    """The layout form pf_groupnorm_train_* read x [B, C, T, H, W] in: "channel" (channels_last_3d, every 8-channel vector
+    16-byte aligned), "plane" (unit-stride (h, w) planes, e.g. NCDHW) or None (neither: the kernels refuse it).  Strides
+    of size-1 axes are ignored, as in the library."""
+    b, c, t, h, w = x.shape
+    s = [0 if n == 1 else st for n, st in zip(x.shape, x.stride())]
+    if (s[1] == 1 and (w == 1 or s[4] == c) and (h == 1 or s[3] == w * c) and s[0] % 8 == 0 and s[2] % 8 == 0
+            and x.data_ptr() % 16 == 0):
+        return "channel"
+    if (w == 1 or s[4] == 1) and (h == 1 or s[3] == w):
+        return "plane"
+    return None
+
+
+def _groupnorm_desc(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, stats: torch.Tensor, groups: int, eps: float,
+                    silu: bool) -> GroupNormTrainDesc:
+    assert x.dtype in (torch.bfloat16, torch.float32) and x.dim() == 5 and x.is_cuda
+    assert gamma.dtype == beta.dtype == stats.dtype == torch.float32 and gamma.is_contiguous() and beta.is_contiguous()
+    b, c, t, h, w = x.shape
+    assert gamma.numel() == beta.numel() == c and stats.is_contiguous() and stats.numel() == b * t * groups * 2
+    d = GroupNormTrainDesc()
+    d.x, d.x_f32 = x.data_ptr(), int(x.dtype == torch.float32)
+    d.b, d.c, d.t, d.h, d.w = b, c, t, h, w
+    for i, st in enumerate(x.stride()):
+        d.x_strides[i] = st
+    d.groups, d.eps, d.silu = groups, eps, int(silu)
+    d.gamma, d.beta, d.stats = gamma.data_ptr(), beta.data_ptr(), stats.data_ptr()
+    return d
+
+
+def _groupnorm_workspace(d: GroupNormTrainDesc, device) -> torch.Tensor:
+    lib = _lib.load()
+    need = int(lib.pf_groupnorm_train_workspace(C.byref(d)))
+    if need < 0:
+        raise RuntimeError(f"libpf_b200 pf_groupnorm_train_workspace failed: {lib.pf_last_error().decode()}")
+    ws = torch.empty(need, device=device, dtype=torch.float32)
+    d.workspace, d.workspace_floats = ws.data_ptr(), need
+    return ws
+
+
+def _dense_in_form(t: torch.Tensor, form: str) -> bool:
+    if form == "channel":
+        return t.permute(0, 2, 3, 4, 1).is_contiguous()
+    return t.is_contiguous()
+
+
+def groupnorm_train_fwd(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, stats: torch.Tensor, y: torch.Tensor, *,
+                        groups: int, eps: float, silu: bool) -> None:
+    """pf_groupnorm_train_fwd: stats fp32 [B*T, groups, 2] = per-frame (mean, rstd) of x [B, C, T, H, W] (bf16 / fp32, channel
+    or plane form); y = act((x - mean) * rstd * gamma + beta), bf16 / fp32, x's shape, dense in x's form."""
+    form = groupnorm_form(x)
+    assert form is not None and y.shape == x.shape and y.dtype in (torch.bfloat16, torch.float32) and _dense_in_form(y, form)
+    d = _groupnorm_desc(x, gamma, beta, stats, groups, eps, silu)
+    d.y, d.y_f32 = y.data_ptr(), int(y.dtype == torch.float32)
+    ws = _groupnorm_workspace(d, x.device)  # noqa: F841  (alive until the launch is queued)
+    _lib.check(_lib.load().pf_groupnorm_train_fwd(C.byref(d), _lib.stream_ptr()), "pf_groupnorm_train_fwd")
+
+
+def groupnorm_train_bwd(x: torch.Tensor, dy: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, stats: torch.Tensor,
+                        dx: Optional[torch.Tensor], dgamma: Optional[torch.Tensor], dbeta: Optional[torch.Tensor], *,
+                        groups: int, silu: bool) -> None:
+    """pf_groupnorm_train_bwd: from dy (x's form, bf16 / fp32) and the forward's stats, dx (x's dtype, dense in x's form) and
+    fp32 dgamma / dbeta [C]; any of the three may be None."""
+    form = groupnorm_form(x)
+    assert form is not None and dy.shape == x.shape and dy.dtype in (torch.bfloat16, torch.float32)
+    assert dx is None or (dx.shape == x.shape and dx.dtype == x.dtype and _dense_in_form(dx, form))
+    for p in (dgamma, dbeta):
+        assert p is None or (p.dtype == torch.float32 and p.is_contiguous() and p.numel() == x.shape[1])
+    d = _groupnorm_desc(x, gamma, beta, stats, groups, 0.0, silu)
+    d.dy, d.dy_f32 = dy.data_ptr(), int(dy.dtype == torch.float32)
+    for i, st in enumerate(dy.stride()):
+        d.dy_strides[i] = st
+    d.dx, d.dgamma, d.dbeta = _ptr(dx), _ptr(dgamma), _ptr(dbeta)
+    ws = _groupnorm_workspace(d, x.device)  # noqa: F841
+    _lib.check(_lib.load().pf_groupnorm_train_bwd(C.byref(d), _lib.stream_ptr()), "pf_groupnorm_train_bwd")

@@ -19,6 +19,20 @@ retain_graph=True before the real backward, video_vae/modeling_loss.py:89-96).
 `install_training_convs(vae)` patches the `forward` of every CausalConv3d of a reference CausalVideoVAE (or of the `.vae`
 of a CausalVideoVAELossWrapper) in place; everything else of the training step -- GroupNorm, SiLU, the mid-block attention,
 the up-samplers' rearranges, LPIPS and the discriminator -- stays torch.  `uninstall_training_convs` restores the instances.
+
+`causal_group_norm(x, weight, bias, num_groups, eps, silu)` is CausalGroupNorm.forward (video_vae/modeling_causal_conv.py:36-43:
+GroupNorm of every (batch, frame)), optionally followed by a SiLU, as an autograd function on pf_groupnorm_train_fwd / _bwd.
+x (bf16 or fp32) is read in place when it is channels_last_3d (what causal_conv3d returns) or has contiguous (h, w) planes
+(NCDHW, the up-samplers' rearranged copies); any other layout is copied to channels_last_3d first (counted in
+`layout_copies`).  The output has x's form; its dtype is fp32 under autocast (torch's group_norm autocasts to fp32) and x's
+dtype otherwise, or `out_dtype`.  Saved are x itself and the fp32 per-frame (mean, rstd); the backward recomputes the
+normalised value, and its partial sums are added in a fixed order (the bits repeat, also under checkpoint recompute).  If a
+saved-tensor hook returns x in other strides (save_on_cpu does), the backward copies it back into the forward's form.  Where
+x has planes and the gradient arrives channels-last (the sites after the up-samplers), the backward repacks a bf16 x
+channels-last with pf_conv3d_pack and runs the channel-form kernels.
+`install_training_norms(vae)` runs every CausalGroupNorm with its following SiLU fused (the SiLU module is replaced by
+nn.Identity on the instance) and, under bf16 autocast, a bf16 output: every such output feeds a conv that rounds its input
+to bf16 anyway.  `uninstall_training_norms` restores the module tree.  The two installs compose in either order.
 """
 from __future__ import annotations
 
@@ -194,4 +208,200 @@ def install_training_convs(vae) -> None:
 def uninstall_training_convs(vae) -> None:
     for _, m in causal_convs(vae):
         if m.__dict__.pop(_MARK, False):
+            del m.forward
+
+
+# ------------------------------------------------------------------------------------------------------------- GroupNorm
+layout_copies = 0     # inputs / gradients causal_group_norm had to copy into a layout the kernels read
+_checked_devices = set()
+
+
+def _require_device_once() -> None:
+    """_lib.require_device() (a cudaGetDeviceProperties, about 3 ms) once per device: the op runs at every norm site."""
+    dev = torch.cuda.current_device()
+    if dev not in _checked_devices:
+        _lib.require_device()
+        _checked_devices.add(dev)
+
+
+def _bf16_autocast() -> bool:
+    return torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda") == torch.bfloat16
+
+
+def _in_form(t: torch.Tensor, form: Optional[str]) -> torch.Tensor:
+    """t in the layout form `form` (or channels_last_3d if form is None / t is in neither form)."""
+    global layout_copies
+    have = ops.groupnorm_form(t)
+    if have is not None and (form is None or have == form):
+        return t
+    layout_copies += 1
+    if form == "plane":
+        return t.contiguous()
+    return t.contiguous(memory_format=torch.channels_last_3d)
+
+
+def _channels_last_for(x: torch.Tensor, dy: torch.Tensor) -> torch.Tensor:
+    """x in channel form when x has planes and dy arrives channels-last (the next conv's data gradient does, at the sites
+    after the up-samplers): a bf16 x with channels a multiple of 64 is repacked by pf_conv3d_pack (an exact, vectorised
+    transposing copy), which is far cheaper than torch's permuting copy of dy into planes."""
+    global layout_copies
+    if not (ops.groupnorm_form(x) == "plane" and ops.groupnorm_form(dy) == "channel" and x.dtype == torch.bfloat16
+            and x.shape[1] % 64 == 0):
+        return x
+    layout_copies += 1
+    b, c, t, h, w = x.shape
+    xc = torch.empty(b, t, h, w, c, device=x.device, dtype=torch.bfloat16)
+    ops.conv3d_pack(x, xc, t_offset=0)
+    return xc.permute(0, 4, 1, 2, 3)
+
+
+def _empty_in_form(like: torch.Tensor, form: str, dtype: torch.dtype) -> torch.Tensor:
+    if form == "channel":
+        b, c, t, h, w = like.shape
+        return torch.empty(b, t, h, w, c, device=like.device, dtype=dtype).permute(0, 4, 1, 2, 3)
+    return torch.empty(like.shape, device=like.device, dtype=dtype)
+
+
+class _CausalGroupNorm(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, weight, bias, groups, eps, silu, out_dtype):
+        x = _in_form(x, None)
+        form = ops.groupnorm_form(x)
+        b, c, t = x.shape[:3]
+        gamma, beta = weight.detach().float().contiguous(), bias.detach().float().contiguous()
+        stats = torch.empty(b * t, groups, 2, device=x.device, dtype=torch.float32)
+        y = _empty_in_form(x, form, out_dtype)
+        ops.groupnorm_train_fwd(x, gamma, beta, stats, y, groups=groups, eps=eps, silu=silu)
+        # through save_for_backward, so that saved-tensor hooks (non-reentrant checkpointing, save_on_cpu) see x and the
+        # statistics; nothing activation-sized besides x is kept
+        ctx.save_for_backward(x, weight, bias, stats)
+        ctx.groups, ctx.silu, ctx.form = groups, silu, form
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, weight, bias, stats = ctx.saved_tensors
+        need_x, need_w, need_b = ctx.needs_input_grad[:3]
+        # a saved-tensor hook may hand x back with other strides than it had in the forward (save_on_cpu unpacks into a
+        # contiguous NCDHW tensor): it is brought back to the forward's form, so the backward runs the same kernels, in the
+        # same summation order, as without the hook
+        x = _in_form(x, ctx.form)
+        x = _channels_last_for(x, dy)
+        form = ops.groupnorm_form(x)
+        dy = _in_form(dy, form)
+        gamma, beta = weight.detach().float().contiguous(), bias.detach().float().contiguous()
+        dx = _empty_in_form(x, form, x.dtype) if need_x else None
+        c = x.shape[1]
+        dgamma = torch.empty(c, device=x.device, dtype=torch.float32) if need_w else None
+        dbeta = torch.empty(c, device=x.device, dtype=torch.float32) if need_b else None
+        ops.groupnorm_train_bwd(x, dy, gamma, beta, stats, dx, dgamma, dbeta, groups=ctx.groups, silu=ctx.silu)
+        if dgamma is not None:
+            dgamma = dgamma.to(weight.dtype)
+        if dbeta is not None:
+            dbeta = dbeta.to(bias.dtype)
+        return dx, dgamma, dbeta, None, None, None, None
+
+
+def causal_group_norm(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, num_groups: int, eps: float,
+                      silu: bool = False, out_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+    """CausalGroupNorm.forward of x [B, C, T, H, W] (then SiLU if `silu`) with an affine GroupNorm's weight / bias.
+    out_dtype None: fp32 under autocast (as torch's group_norm), x's dtype otherwise."""
+    if x.dim() != 5 or weight is None or bias is None or weight.shape != (x.shape[1],) or bias.shape != (x.shape[1],):
+        raise ValueError(f"causal_group_norm: x {tuple(x.shape)} is not [B, C, T, H, W] with an affine weight / bias of C")
+    if x.dtype not in (torch.bfloat16, torch.float32):
+        raise TypeError(f"causal_group_norm: x must be bf16 or fp32, got {x.dtype}")
+    c = x.shape[1]
+    if c % 8 or c % num_groups:
+        raise ValueError(f"causal_group_norm: {c} channels must be a multiple of 8 and of num_groups={num_groups}")
+    if not (x.is_cuda and weight.is_cuda and bias.is_cuda):
+        raise RuntimeError("causal_group_norm runs on the library's CUDA kernels: x, weight and bias must be CUDA tensors "
+                           "(there is no CPU path)")
+    if out_dtype is None:
+        out_dtype = torch.float32 if torch.is_autocast_enabled("cuda") else x.dtype
+    if out_dtype not in (torch.bfloat16, torch.float32):
+        raise TypeError(f"causal_group_norm: out_dtype must be bf16 or fp32, got {out_dtype}")
+    _require_device_once()
+    return _CausalGroupNorm.apply(x, weight, bias, int(num_groups), float(eps), bool(silu), out_dtype)
+
+
+# ---------------------------------------------------------------------------------------------------------------- drop-in
+_NORM_MARK = "_pf_training_norm"
+_SAVED_ACT = "_pf_saved_activation"
+
+
+def causal_group_norms(vae) -> List[Tuple[str, nn.Module]]:
+    """(name, module) of every reference CausalGroupNorm under a CausalVideoVAE or a CausalVideoVAELossWrapper's `.vae`."""
+    return [(n, m) for n, m in _target(vae).named_modules()
+            if type(m).__name__ == "CausalGroupNorm" and isinstance(m, nn.GroupNorm)]
+
+
+def _norm_sites(vae):
+    """(owner, activation attribute, [its CausalGroupNorms]) for every norm -> SiLU pair the install fuses:
+    CausalResnetBlock3D norm1 / norm2 -> nonlinearity, and the encoder's / decoder's conv_norm_out -> conv_act."""
+    sites = []
+    for name, m in _target(vae).named_modules():
+        if type(m).__name__ == "CausalResnetBlock3D":
+            sites.append((name, m, "nonlinearity", [getattr(m, "norm1", None), getattr(m, "norm2", None)]))
+        elif type(getattr(m, "conv_norm_out", None)).__name__ == "CausalGroupNorm" and hasattr(m, "conv_act"):
+            sites.append((name, m, "conv_act", [m.conv_norm_out]))
+    return sites
+
+
+def _norm_refusal(name: str, owner: nn.Module, act_attr: str, norms) -> Optional[str]:
+    act = owner.__dict__.get(_SAVED_ACT, getattr(owner, act_attr))
+    if type(act) is not nn.SiLU:
+        return f"{name}.{act_attr} is {type(act).__name__}, not nn.SiLU"
+    if act_attr == "nonlinearity":
+        if getattr(owner, "time_embedding_norm", "default") != "default":
+            return f"{name}: time_embedding_norm {owner.time_embedding_norm!r} is not 'default'"
+        drop = getattr(owner, "dropout", None)
+        if drop is not None and getattr(drop, "p", 0.0) > 0:
+            return f"{name}: dropout p={drop.p} sits between the norm's bf16 output and conv2"
+    for n in norms:
+        if type(n).__name__ != "CausalGroupNorm":
+            return f"{name}: {type(n).__name__} before the {act_attr} is not a CausalGroupNorm"
+        if not n.affine:
+            return f"{name}: a CausalGroupNorm without affine parameters"
+        if n.num_channels % 8:
+            return f"{name}: {n.num_channels} channels are not a multiple of 8"
+    return None
+
+
+def _patched_norm_forward(self, x):
+    return causal_group_norm(x, self.weight, self.bias, self.num_groups, self.eps, silu=True,
+                             out_dtype=torch.bfloat16 if _bf16_autocast() else None)
+
+
+def install_training_norms(vae) -> None:
+    """Run every CausalGroupNorm of a reference CausalVideoVAE (or CausalVideoVAELossWrapper) on `causal_group_norm` with
+    the SiLU after it fused; the SiLU module becomes nn.Identity on its owner."""
+    norms = causal_group_norms(vae)
+    if not norms:
+        raise ValueError("no CausalGroupNorm found: pass a reference CausalVideoVAE or CausalVideoVAELossWrapper")
+    sites = _norm_sites(vae)
+    covered = set()
+    for name, owner, act_attr, site_norms in sites:
+        why = _norm_refusal(name, owner, act_attr, site_norms)
+        if why is not None:
+            raise ValueError(f"install_training_norms: {why}")
+        covered.update(id(n) for n in site_norms)
+    for name, m in norms:
+        if id(m) not in covered:
+            raise ValueError(f"install_training_norms: {name} is not followed by a SiLU the install knows how to fuse")
+    for _, owner, act_attr, site_norms in sites:
+        if _SAVED_ACT not in owner.__dict__:
+            owner.__dict__[_SAVED_ACT] = getattr(owner, act_attr)     # kept off the module tree and the state_dict
+            setattr(owner, act_attr, nn.Identity())
+        for n in site_norms:
+            n.forward = types.MethodType(_patched_norm_forward, n)
+            setattr(n, _NORM_MARK, True)
+
+
+def uninstall_training_norms(vae) -> None:
+    for _, owner, act_attr, _ in _norm_sites(vae):
+        act = owner.__dict__.pop(_SAVED_ACT, None)
+        if act is not None:
+            setattr(owner, act_attr, act)
+    for _, m in causal_group_norms(vae):
+        if m.__dict__.pop(_NORM_MARK, False):
             del m.forward
