@@ -492,6 +492,14 @@ typedef struct pf_conv3d_desc {
                                          * stay OUTPUT dims; x is [B, (t-1)*stride_t + kt, h*stride_h, w*stride_w, cin]. */
   int32_t kernel_variant; /* 0 = auto; 1 = 128-wide filter tiles (cout % 128 == 0); 2 = 64-wide filter tiles.
                            * Both accumulate in the same K order: the choice never changes the bits. */
+  /* Plain-store epilogues of the LPIPS VGG16 (torchvision vgg16().features, video_vae/modeling_lpips.py:67-104), where a
+   * 3x3 pad-1 Conv2d is this conv with kt = 1 on T = 1.  Both 0 (the default) = the behaviour and bits above.  Neither may
+   * be combined with a residual, with store modes 1 / 2, or with the other. */
+  int32_t relu;       /* 1: store max(x, 0) after the bias (conv + ReLU(inplace=True)) */
+  const void* select; /* bf16, addressed like residual (res_t_total / res_t_offset, out_c channels, out_c % 16 == 0,
+                       * store_channels == out_c): store select > 0 ? x : 0.  With select = the ReLU output of the layer
+                       * in front, this is the data gradient with that ReLU's backward (threshold_backward) fused: a select,
+                       * so a non-finite x is dropped where the ReLU output is 0. */
 } pf_conv3d_desc;
 PF_API int pf_causal_conv3d(const pf_conv3d_desc* desc, void* stream);
 
@@ -608,6 +616,65 @@ typedef struct pf_groupnorm_train_desc {
 PF_API int64_t pf_groupnorm_train_workspace(const pf_groupnorm_train_desc* desc);
 PF_API int pf_groupnorm_train_fwd(const pf_groupnorm_train_desc* desc, void* stream);
 PF_API int pf_groupnorm_train_bwd(const pf_groupnorm_train_desc* desc, void* stream);
+/* ------------------------------------------------------------------ LPIPS (VAE training loss)
+ * LPIPS.forward (video_vae/modeling_lpips.py:32-45) as LPIPSWithDiscriminator runs it on every generator step
+ * (video_vae/modeling_loss.py:123): ScalingLayer (:48-56), vgg16().features[:30] (:67-104: 13 conv3x3 + ReLU, MaxPool2d(2, 2)
+ * in front of slices 2-5), and at each of the 5 taps normalize_tensor (:107-110), (f0 - f1)^2, lin_k = Dropout(0.5) + a
+ * bias-free 1x1 Conv2d(C, 1) (NetLinLayer :58-65), spatial_average (:112-113), summed over the taps.  The convs are
+ * pf_causal_conv3d with kt = 1 on T = 1 (relu / select epilogues); every tensor below is channels-last bf16 [n, h, w, c].
+ *
+ * pf_maxpool2x2: y [n, h/2, w/2, c] = max over each 2x2 window of x [n, h, w, c] (h, w even, c % 8 == 0, 16-byte aligned).
+ * pf_maxpool2x2_bwd: dx [n, h, w, c] = dy [n, h/2, w/2, c] at the window's first maximum in row-major order (torch's
+ *   max_pool2d scan: an element wins when it is greater than every earlier one, or NaN), 0 elsewhere.  Both are exact.
+ *
+ * Dropout (nn.Dropout in training mode): element (tap k, image i, pixel p, channel c) is kept iff
+ *   (Philox4x32-10(counter = (c / 4, i * h * w + p, k, 0), key = seed)[c % 4] >> 8) * 2^-24 >= p, and scaled by 1 / (1 - p);
+ *   seed is an int64 on the device (drawn from torch's CUDA generator per call, so nothing syncs).  p = 0: no dropout
+ *   (eval mode), seed may be NULL.  The kernels recompute the mask; nothing is stored. */
+#define PF_LPIPS_MAX_TAPS 5
+#define PF_LPIPS_HEAD_BLOCKS 32
+/* pf_lpips_head_fwd: val fp32 [n] = sum_k 1/(h_k w_k) sum_pixels sum_c lin_k[c] keep (f0^ - f1^)_c^2 with
+ *   f^ = f / (sqrt(sum_c f^2) + 1e-10), in fp32 from the bf16 taps; c_k in {64, 128, 256, 512}.  Each (image, tap) is summed by
+ *   PF_LPIPS_HEAD_BLOCKS blocks into workspace (>= taps * n * PF_LPIPS_HEAD_BLOCKS floats), then added in a fixed order. */
+typedef struct pf_lpips_head_desc {
+  int32_t n, taps;
+  const void* f0[PF_LPIPS_MAX_TAPS]; /* branch 0 (LPIPS's `input`) taps */
+  const void* f1[PF_LPIPS_MAX_TAPS]; /* branch 1 (`target`) taps */
+  const float* lin[PF_LPIPS_MAX_TAPS]; /* fp32 [c_k]: lin_k's 1x1 conv weight */
+  int32_t c[PF_LPIPS_MAX_TAPS], h[PF_LPIPS_MAX_TAPS], w[PF_LPIPS_MAX_TAPS];
+  float p;
+  const int64_t* seed;
+  float* val;
+  float* workspace;
+  int64_t workspace_floats;
+} pf_lpips_head_desc;
+PF_API int pf_lpips_head_fwd(const pf_lpips_head_desc* desc, void* stream);
+/* pf_lpips_tap_bwd: at tap `tap` for one branch with features f (this branch) and f_other, given grad fp32 [n] = dLoss/dval:
+ *   dz = f > 0 ? head_grad + route(d_next) : 0, summed in fp32 and rounded once to bf16, where
+ *   head_grad = the gradient of val through normalize_tensor (0 where |f| = 0: the ReLU select drops it in the reference,
+ *               whose sqrt backward is NaN there) with the same dropout bits as the forward, and
+ *   route(d_next) = pf_maxpool2x2_bwd of d_next [n, h/2, w/2, c] (the next slice's first-conv data gradient; NULL at the
+ *               last tap).
+ * This is the ReLU backward of the tap's conv, fused with the head and the pool backward: dz is the gradient of that conv's
+ * output, the input of its data gradient. */
+typedef struct pf_lpips_tap_bwd_desc {
+  int32_t n, c, h, w, tap;
+  const void* f;
+  const void* f_other;
+  const float* lin;
+  float p;
+  const int64_t* seed;
+  const float* grad;
+  const void* d_next;
+  void* dz;
+} pf_lpips_tap_bwd_desc;
+PF_API int pf_lpips_tap_bwd(const pf_lpips_tap_bwd_desc* desc, void* stream);
+PF_API int pf_maxpool2x2(const void* x, void* y, int32_t n, int32_t h, int32_t w, int32_t c, void* stream);
+PF_API int pf_maxpool2x2_bwd(const void* x, const void* dy, void* dx, int32_t n, int32_t h, int32_t w, int32_t c, void* stream);
+/* the keep mask (uint8 1 / 0, [n, h, w, c], 8-byte aligned) the head draws at (seed, tap) for dropout p: for tests */
+PF_API int pf_lpips_dropout_mask(const int64_t* seed, int32_t tap, int32_t n, int32_t h, int32_t w, int32_t c, float p,
+                                 uint8_t* mask, void* stream);
+
 /* in-place row softmax of bf16 scores [rows, ld]: softmax over the first `cols` columns of scale*s, zeros in the padding
  * (mid-block attention, diffusers Attention used at K:454-460). */
 PF_API int pf_softmax_rows(void* s_bf16, int64_t rows, int32_t cols, int64_t ld, float scale, void* stream);

@@ -29,6 +29,7 @@ SYMBOLS = [
     "pf_attn_fwd_text", "pf_rms_norm_rows", "pf_embed_tokens",
     "pf_conv3d_pack", "pf_conv3d_wgrad_workspace", "pf_conv3d_wgrad",
     "pf_groupnorm_train_workspace", "pf_groupnorm_train_fwd", "pf_groupnorm_train_bwd",
+    "pf_maxpool2x2", "pf_maxpool2x2_bwd", "pf_lpips_head_fwd", "pf_lpips_tap_bwd", "pf_lpips_dropout_mask",
 ]
 
 PF_OPT_GEMM_STAGED_RESID, PF_OPT_GEMM_WAVE_TILING, PF_OPT_ATTN_PAIR_KERNEL, PF_OPT_ATTN_TILE_PHASE, PF_OPT_ATTN_TRIPLE_KERNEL = range(5)
@@ -150,6 +151,7 @@ class ConvDesc(C.Structure):
         ("store_channels", C.c_int32),
         ("residual", C.c_void_p), ("res_t_total", C.c_int32), ("res_t_offset", C.c_int32),
         ("stride_t", C.c_int32), ("stride_h", C.c_int32), ("stride_w", C.c_int32), ("kernel_variant", C.c_int32),
+        ("relu", C.c_int32), ("select", C.c_void_p),
     ]
 
 
@@ -186,6 +188,29 @@ class GroupNormTrainDesc(C.Structure):
         ("dy", C.c_void_p), ("dy_f32", C.c_int32), ("dy_strides", C.c_int64 * 5),
         ("dx", C.c_void_p), ("dgamma", C.c_void_p), ("dbeta", C.c_void_p),
         ("workspace", C.c_void_p), ("workspace_floats", C.c_int64),
+    ]
+
+
+LPIPS_MAX_TAPS = 5          # PF_LPIPS_MAX_TAPS
+LPIPS_HEAD_BLOCKS = 32      # PF_LPIPS_HEAD_BLOCKS
+
+
+class LpipsHeadDesc(C.Structure):
+    _fields_ = [
+        ("n", C.c_int32), ("taps", C.c_int32),
+        ("f0", C.c_void_p * LPIPS_MAX_TAPS), ("f1", C.c_void_p * LPIPS_MAX_TAPS), ("lin", C.c_void_p * LPIPS_MAX_TAPS),
+        ("c", C.c_int32 * LPIPS_MAX_TAPS), ("h", C.c_int32 * LPIPS_MAX_TAPS), ("w", C.c_int32 * LPIPS_MAX_TAPS),
+        ("p", C.c_float), ("seed", C.c_void_p), ("val", C.c_void_p),
+        ("workspace", C.c_void_p), ("workspace_floats", C.c_int64),
+    ]
+
+
+class LpipsTapBwdDesc(C.Structure):
+    _fields_ = [
+        ("n", C.c_int32), ("c", C.c_int32), ("h", C.c_int32), ("w", C.c_int32), ("tap", C.c_int32),
+        ("f", C.c_void_p), ("f_other", C.c_void_p), ("lin", C.c_void_p),
+        ("p", C.c_float), ("seed", C.c_void_p), ("grad", C.c_void_p),
+        ("d_next", C.c_void_p), ("dz", C.c_void_p),
     ]
 
 
@@ -266,6 +291,13 @@ def load() -> C.CDLL:
         getattr(lib, name).argtypes = [C.POINTER(GroupNormTrainDesc), C.c_void_p]
     lib.pf_groupnorm_train_workspace.argtypes = [C.POINTER(GroupNormTrainDesc)]
     lib.pf_groupnorm_train_workspace.restype = C.c_int64
+    lib.pf_lpips_head_fwd.argtypes = [C.POINTER(LpipsHeadDesc), C.c_void_p]
+    lib.pf_lpips_tap_bwd.argtypes = [C.POINTER(LpipsTapBwdDesc), C.c_void_p]
+    lib.pf_maxpool2x2.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
+    lib.pf_maxpool2x2_bwd.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                      C.c_void_p]
+    lib.pf_lpips_dropout_mask.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float,
+                                          C.c_void_p, C.c_void_p]
     lib.pf_groupnorm_stats.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_float, C.c_void_p,
                                        C.c_void_p, C.c_int64, C.c_void_p]
     lib.pf_groupnorm_apply.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32,

@@ -10,8 +10,9 @@
 //   B tile  = weights re-laid out as [Cout, taps*Cin] (tap-major), a plain 2-D TMA box like the GEMM.
 // The box lands in shared memory as [TH][TW][64] = 128 rows of 128 B with SWIZZLE_128B, i.e. exactly the K-major wgmma
 // operand; no im2col buffer exists anywhere.  Pipeline / warp roles are the GEMM's (pf_gemm.cu).
-// Epilogue: bias (+ residual) -> bf16/fp32 channels-last store, optionally through the depth-to-space addressing of
-// CausalUpsample2x (R:616) / CausalTemporalUpsample2x (R:724-727) so the rearrange copy disappears.
+// Epilogue: bias (+ residual, or a ReLU, or the select of a ReLU backward) -> bf16/fp32 channels-last store, optionally
+// through the depth-to-space addressing of CausalUpsample2x (R:616) / CausalTemporalUpsample2x (R:724-727) so the
+// rearrange copy disappears.
 #include <cstdlib>
 
 #include "../../include/pf_b200.h"
@@ -34,6 +35,8 @@ struct ConvArgs {
   int store_channels;  // channels of the conv output that are stored (<= cout; the rest is padding)
   const __nv_bfloat16* residual;   // plain mode only; same geometry as out (bf16)
   int res_t_total, res_t_offset;
+  int relu;                        // plain mode, no residual: store max(x, 0)
+  const __nv_bfloat16* select;     // plain mode, no residual: store select > 0 ? x : 0 (select addressed like residual)
 };
 
 constexpr int CBK = PIPE_BK;
@@ -72,6 +75,25 @@ __device__ __forceinline__ void conv_epilogue_tile(const ConvArgs& g, const floa
             const float2 f = __bfloat1622float2(hv[i]);
             x[8 * u + 2 * i] += f.x;
             x[8 * u + 2 * i + 1] += f.y;
+          }
+        }
+      }
+      if (g.relu) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) x[i] = fmaxf(x[i], 0.f);
+      } else if (g.select != nullptr) {
+        // the ReLU backward of the layer whose output `select` is: a select, so a non-finite x never leaks where select <= 0
+        const size_t svox = ((static_cast<size_t>(bb) * g.res_t_total + (tt + g.res_t_offset)) * g.out_h + hh) * g.out_w + ww;
+        const uint4* s4 = reinterpret_cast<const uint4*>(g.select + svox * g.out_c + n0);
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const uint4 sv = __ldg(s4 + u);
+          const __nv_bfloat162* hv = reinterpret_cast<const __nv_bfloat162*>(&sv);
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const float2 f = __bfloat1622float2(hv[i]);
+            x[8 * u + 2 * i] = f.x > 0.f ? x[8 * u + 2 * i] : 0.f;
+            x[8 * u + 2 * i + 1] = f.y > 0.f ? x[8 * u + 2 * i + 1] : 0.f;
           }
         }
       }
@@ -272,6 +294,10 @@ extern "C" int pf_causal_conv3d(const pf_conv3d_desc* d, void* stream_) {
   if (d->store_mode == 2) PF_REQUIRE(d->store_channels == d->cout && d->out_c * 2 == d->cout && !d->out_f32 && !d->residual, "pf_causal_conv3d: temporal depth-to-space needs out_c = cout/2, bf16, no residual");
   if (d->store_mode == 0) PF_REQUIRE(d->out_c >= d->store_channels, "pf_causal_conv3d: out_c < store_channels");
   PF_REQUIRE(d->out_f32 >= 0 && d->out_f32 <= 2 && (d->out_f32 != 2 || !d->residual), "pf_causal_conv3d: out_f32 must be 0 (bf16), 1 (fp32) or 2 (uint8 image, no residual)");
+  PF_REQUIRE(d->relu == 0 || d->relu == 1, "pf_causal_conv3d: relu must be 0 or 1");
+  if (d->relu || d->select)
+    PF_REQUIRE(d->store_mode == 0 && !d->residual && !(d->relu && d->select), "pf_causal_conv3d: relu and select are plain-store epilogues, one at a time, without a residual");
+  if (d->select) PF_REQUIRE(d->out_c % 16 == 0 && d->store_channels == d->out_c && (reinterpret_cast<uintptr_t>(d->select) & 15) == 0, "pf_causal_conv3d: select needs out_c %% 16 == 0, store_channels == out_c and a 16-byte aligned tensor");
   const int st = d->stride_t > 1 ? d->stride_t : 1, sh = d->stride_h > 1 ? d->stride_h : 1, sw = d->stride_w > 1 ? d->stride_w : 1;
   PF_REQUIRE(st <= 2 && sh <= 2 && sw <= 2 && sh == sw, "pf_causal_conv3d: strides must be 1 or 2 with stride_h == stride_w");
   if (st > 1 || sh > 1) PF_REQUIRE(d->store_mode == 0 && d->kt == 3 && d->kh == 3, "pf_causal_conv3d: strided convs are plain-store 3x3x3 (CausalDownsample2x R:322, CausalTemporalDownsample2x R:486)");
@@ -296,6 +322,8 @@ extern "C" int pf_causal_conv3d(const pf_conv3d_desc* d, void* stream_) {
   g.store_channels = d->store_channels;
   g.residual = static_cast<const __nv_bfloat16*>(d->residual);
   g.res_t_total = d->res_t_total; g.res_t_offset = d->res_t_offset;
+  g.relu = d->relu;
+  g.select = static_cast<const __nv_bfloat16*>(d->select);
 
   // kernel_variant 1 / 2 pins the 128-wide / 64-wide filter tile (same K order, same bits)
   PF_REQUIRE(d->kernel_variant >= 0 && d->kernel_variant <= 2, "pf_causal_conv3d: bad kernel_variant %d", d->kernel_variant);

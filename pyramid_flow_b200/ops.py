@@ -11,8 +11,8 @@ import torch
 
 from . import _lib
 from ._lib import (AttnBwdDesc, AttnDesc, AttnPackDesc, AttnTextDesc, AttnVarlenPackDesc, AttnVarlenUnpackDesc, ConvDesc,
-                   ConvPackDesc, ConvWgradDesc, GemmDesc, GroupNormTrainDesc, PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_GELU,
-                   PF_EPI_QKV_ROPE, PF_EPI_STORE_BF16, PF_EPI_STORE_F32)
+                   ConvPackDesc, ConvWgradDesc, GemmDesc, GroupNormTrainDesc, LpipsHeadDesc, LpipsTapBwdDesc,
+                   PF_EPI_GATE_RESID, PF_EPI_GELU_BF16, PF_EPI_QKV_GELU, PF_EPI_QKV_ROPE, PF_EPI_STORE_BF16, PF_EPI_STORE_F32)
 
 
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
@@ -613,9 +613,11 @@ def conv3d_pack(src: torch.Tensor, dst: torch.Tensor, *, t_offset: int, dil=(1, 
 
 
 def causal_conv3d(x: torch.Tensor, wgt: torch.Tensor, bias: Optional[torch.Tensor], out: torch.Tensor, *, kernel, stride=(1, 1, 1),
-                  store_channels: Optional[int] = None) -> None:
+                  store_channels: Optional[int] = None, relu: bool = False,
+                  select: Optional[torch.Tensor] = None) -> None:
     """pf_causal_conv3d, plain store.  x bf16 [B, (t-1)*st + kt, h*sh, w*sw, cin_p] (packed, causal frames in front);
-    wgt bf16 [cout_p, taps*cin_p]; bias fp32 [cout_p] or None; out bf16 / fp32 [B, t, h, w, out_c] (the output dims)."""
+    wgt bf16 [cout_p, taps*cin_p]; bias fp32 [cout_p] or None; out bf16 / fp32 [B, t, h, w, out_c] (the output dims).
+    relu: store max(y, 0); select (bf16, out's shape): store select > 0 ? y : 0."""
     kt, kh, kw = kernel
     st, sh, sw = stride
     b, t, h, w, out_c = out.shape
@@ -632,6 +634,10 @@ def causal_conv3d(x: torch.Tensor, wgt: torch.Tensor, bias: Optional[torch.Tenso
     d.out_t_total, d.out_t_offset, d.out_c = t, 0, out_c
     d.store_channels = out_c if store_channels is None else store_channels
     d.stride_t, d.stride_h, d.stride_w = st, sh, sw
+    d.relu = int(relu)
+    if select is not None:
+        assert select.dtype == torch.bfloat16 and select.is_contiguous() and select.shape == out.shape
+        d.select, d.res_t_total, d.res_t_offset = select.data_ptr(), t, 0
     _lib.check(_lib.load().pf_causal_conv3d(C.byref(d), _lib.stream_ptr()), "pf_causal_conv3d")
 
 
@@ -732,3 +738,79 @@ def groupnorm_train_bwd(x: torch.Tensor, dy: torch.Tensor, gamma: torch.Tensor, 
     d.dx, d.dgamma, d.dbeta = _ptr(dx), _ptr(dgamma), _ptr(dbeta)
     ws = _groupnorm_workspace(d, x.device)  # noqa: F841
     _lib.check(_lib.load().pf_groupnorm_train_bwd(C.byref(d), _lib.stream_ptr()), "pf_groupnorm_train_bwd")
+
+
+# ---- LPIPS (channels-last bf16 [N, H, W, C] feature maps; see include/pf_b200.h) --------------------------------------------
+def _nhwc_bf16(t: torch.Tensor) -> None:
+    assert t.dtype == torch.bfloat16 and t.is_contiguous() and t.dim() == 4 and t.is_cuda
+
+
+def maxpool2x2(x: torch.Tensor, y: torch.Tensor) -> None:
+    """pf_maxpool2x2: y [N, H/2, W/2, C] = MaxPool2d(2, 2) of x [N, H, W, C]."""
+    _nhwc_bf16(x), _nhwc_bf16(y)
+    n, h, w, c = x.shape
+    assert y.shape == (n, h // 2, w // 2, c)
+    _lib.check(_lib.load().pf_maxpool2x2(x.data_ptr(), y.data_ptr(), n, h, w, c, _lib.stream_ptr()), "pf_maxpool2x2")
+
+
+def maxpool2x2_bwd(x: torch.Tensor, dy: torch.Tensor, dx: torch.Tensor) -> None:
+    """pf_maxpool2x2_bwd: dx [N, H, W, C] = dy [N, H/2, W/2, C] routed to each window's first maximum of x."""
+    _nhwc_bf16(x), _nhwc_bf16(dy), _nhwc_bf16(dx)
+    n, h, w, c = x.shape
+    assert dx.shape == x.shape and dy.shape == (n, h // 2, w // 2, c)
+    _lib.check(_lib.load().pf_maxpool2x2_bwd(x.data_ptr(), dy.data_ptr(), dx.data_ptr(), n, h, w, c, _lib.stream_ptr()),
+               "pf_maxpool2x2_bwd")
+
+
+def lpips_head_fwd(f0, f1, lin, val: torch.Tensor, *, p: float = 0.0, seed: Optional[torch.Tensor] = None) -> None:
+    """pf_lpips_head_fwd: val fp32 [N] = sum over the taps of the spatial mean of lin_k . dropout((f0^ - f1^)^2).
+    f0, f1: sequences of the taps' feature maps; lin: fp32 [C_k] weights; seed: int64 [1] on the device (p > 0)."""
+    assert len(f0) == len(f1) == len(lin) and 1 <= len(f0) <= _lib.LPIPS_MAX_TAPS
+    assert val.dtype == torch.float32 and val.is_contiguous() and val.numel() == f0[0].shape[0]
+    d = LpipsHeadDesc()
+    d.n, d.taps = f0[0].shape[0], len(f0)
+    for k, (a, b, wl) in enumerate(zip(f0, f1, lin)):
+        _nhwc_bf16(a), _nhwc_bf16(b)
+        assert a.shape == b.shape and a.shape[0] == d.n
+        assert wl.dtype == torch.float32 and wl.is_contiguous() and wl.numel() == a.shape[3]
+        d.f0[k], d.f1[k], d.lin[k] = a.data_ptr(), b.data_ptr(), wl.data_ptr()
+        d.h[k], d.w[k], d.c[k] = a.shape[1:]
+    d.p, d.seed, d.val = p, _seed_ptr(seed, p), val.data_ptr()
+    ws = torch.empty(d.taps * d.n * _lib.LPIPS_HEAD_BLOCKS, device=val.device, dtype=torch.float32)
+    d.workspace, d.workspace_floats = ws.data_ptr(), ws.numel()
+    _lib.check(_lib.load().pf_lpips_head_fwd(C.byref(d), _lib.stream_ptr()), "pf_lpips_head_fwd")
+
+
+def lpips_tap_bwd(f: torch.Tensor, f_other: torch.Tensor, lin: torch.Tensor, grad: torch.Tensor, d_next: Optional[torch.Tensor],
+                  dz: torch.Tensor, *, tap: int, p: float = 0.0, seed: Optional[torch.Tensor] = None) -> None:
+    """pf_lpips_tap_bwd: dz = f > 0 ? (head gradient at tap `tap` + max-pool route of d_next) : 0, for the branch of f;
+    grad fp32 [N] = the gradient of the head's value; d_next [N, H/2, W/2, C] or None."""
+    for t in (f, f_other, dz):
+        _nhwc_bf16(t)
+    assert f.shape == f_other.shape == dz.shape
+    n, h, w, c = f.shape
+    assert lin.dtype == torch.float32 and lin.is_contiguous() and lin.numel() == c
+    assert grad.dtype == torch.float32 and grad.is_contiguous() and grad.numel() == n
+    if d_next is not None:
+        _nhwc_bf16(d_next)
+        assert d_next.shape == (n, h // 2, w // 2, c)
+    d = LpipsTapBwdDesc()
+    d.n, d.c, d.h, d.w, d.tap = n, c, h, w, tap
+    d.f, d.f_other, d.lin, d.p, d.seed = f.data_ptr(), f_other.data_ptr(), lin.data_ptr(), p, _seed_ptr(seed, p)
+    d.grad, d.d_next, d.dz = grad.data_ptr(), _ptr(d_next), dz.data_ptr()
+    _lib.check(_lib.load().pf_lpips_tap_bwd(C.byref(d), _lib.stream_ptr()), "pf_lpips_tap_bwd")
+
+
+def lpips_dropout_mask(seed: torch.Tensor, mask: torch.Tensor, *, tap: int, p: float) -> None:
+    """pf_lpips_dropout_mask: mask uint8 [N, H, W, C] = 1 where the head keeps the element at (seed, tap), else 0."""
+    assert mask.dtype == torch.uint8 and mask.is_contiguous() and mask.dim() == 4
+    n, h, w, c = mask.shape
+    _lib.check(_lib.load().pf_lpips_dropout_mask(_seed_ptr(seed, p), tap, n, h, w, c, p, mask.data_ptr(), _lib.stream_ptr()),
+               "pf_lpips_dropout_mask")
+
+
+def _seed_ptr(seed: Optional[torch.Tensor], p: float) -> Optional[int]:
+    if seed is None:
+        return None
+    assert seed.dtype == torch.int64 and seed.is_cuda and seed.numel() >= 1
+    return seed.data_ptr()

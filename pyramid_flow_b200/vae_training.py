@@ -33,10 +33,18 @@ channels-last with pf_conv3d_pack and runs the channel-form kernels.
 `install_training_norms(vae)` runs every CausalGroupNorm with its following SiLU fused (the SiLU module is replaced by
 nn.Identity on the instance) and, under bf16 autocast, a bf16 output: every such output feeds a conv that rounds its input
 to bf16 anyway.  `uninstall_training_norms` restores the module tree.  The two installs compose in either order.
+
+`lpips(input, target, module)` is LPIPS.forward (video_vae/modeling_lpips.py:32-45) of a reference LPIPS module, an autograd
+function: ScalingLayer in fp32 torch ops, the 13 VGG16 convs on pf_causal_conv3d (kt = 1, ReLU fused), pf_maxpool2x2, and
+pf_lpips_head_fwd over the five taps (dropout from the lin layers' Dropout when it is in training mode); the backward runs
+pf_lpips_tap_bwd at the taps and the data-gradient convs with the ReLU select.  The output is fp32 [N, 1, 1, 1].
+`install_training_lpips(model)` patches the LPIPS of a CausalVideoVAELossWrapper / LPIPSWithDiscriminator / LPIPS;
+`uninstall_training_lpips` restores it.  The three installs compose in any order.
 """
 from __future__ import annotations
 
 import types
+import weakref
 from typing import List, Optional, Tuple
 
 import torch
@@ -405,3 +413,244 @@ def uninstall_training_norms(vae) -> None:
     for _, m in causal_group_norms(vae):
         if m.__dict__.pop(_NORM_MARK, False):
             del m.forward
+
+
+# ------------------------------------------------------------------------------------------------------------------ LPIPS
+# vgg16().features[:30] as LPIPS slices it (video_vae/modeling_lpips.py:67-89): (in, out) of the 13 conv3x3 + ReLU, the
+# convs per slice, a MaxPool2d(2, 2) in front of slices 2-5; the five slice outputs are the taps relu1_2 ... relu5_3.
+VGG16_CONVS = ((3, 64), (64, 64), (64, 128), (128, 128), (128, 256), (256, 256), (256, 256), (256, 512), (512, 512),
+               (512, 512), (512, 512), (512, 512), (512, 512))
+VGG16_SLICES = (2, 2, 3, 3, 3)
+_LPIPS_MARK = "_pf_training_lpips"
+_lpips_filters = {}
+
+
+def _frozen_layout(weight: torch.Tensor, kind: str, build):
+    """A re-layout of a frozen weight, built once per (tensor, in-place version).  The entry holds a weak reference to the
+    tensor, so a new tensor at a freed tensor's address is never served the old layout."""
+    key = (kind, weight.device, weight.data_ptr(), tuple(weight.shape))
+    hit = _lpips_filters.get(key)
+    if hit is None or hit[0]() is not weight or hit[1] != weight._version:
+        hit = _lpips_filters[key] = (weakref.ref(weight), weight._version, build(weight))
+    return hit[2]
+
+
+def _vgg_filter(weight: torch.Tensor) -> torch.Tensor:
+    return _frozen_layout(weight, "fwd", lambda w: forward_filter(w.unsqueeze(2), _pad64(w.shape[0]), _pad64(w.shape[1])))
+
+
+def _vgg_dgrad_filter(weight: torch.Tensor) -> torch.Tensor:
+    return _frozen_layout(weight, "dgrad", lambda w: dgrad_filter(w.unsqueeze(2), _pad64(w.shape[0]), _pad64(w.shape[1])))
+
+
+def _vgg_bias(bias: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+    return None if bias is None else _frozen_layout(bias, "bias", lambda b: b.detach().float().contiguous())
+
+
+def _lin_weight(conv: nn.Conv2d) -> torch.Tensor:
+    return _frozen_layout(conv.weight, "lin", lambda w: w.detach().float().reshape(-1).contiguous())
+
+
+def _vgg_modules(lp: nn.Module) -> List[List[nn.Module]]:
+    net = getattr(lp, "net", None)
+    return [list(getattr(net, f"slice{s + 1}", nn.Sequential()).children()) for s in range(5)]
+
+
+def _lin_layers(lp: nn.Module) -> List[nn.Sequential]:
+    return [getattr(getattr(lp, f"lin{k}", None), "model", None) for k in range(5)]
+
+
+def _lpips_refusal(lp: nn.Module) -> Optional[str]:
+    trainable = [n for n, p in lp.named_parameters() if p.requires_grad]
+    if trainable:
+        return f"parameters {trainable[:3]} require grad (the op computes no LPIPS weight gradient)"
+    sl = getattr(lp, "scaling_layer", None)
+    if sl is None or getattr(sl, "shift", None) is None or sl.shift.numel() != 3 or sl.scale.numel() != 3:
+        return "no ScalingLayer with 3-channel shift / scale buffers"
+    ci = 0
+    for s, mods in enumerate(_vgg_modules(lp)):
+        want = 2 * VGG16_SLICES[s] + (s > 0)
+        if len(mods) != want:
+            return f"net.slice{s + 1} has {len(mods)} modules, not the {want} of vgg16().features"
+        if s > 0:
+            pool = mods[0]
+            if not (type(pool) is nn.MaxPool2d and pool.kernel_size in (2, (2, 2)) and pool.stride in (2, (2, 2))
+                    and pool.padding in (0, (0, 0)) and pool.dilation in (1, (1, 1)) and not pool.ceil_mode):
+                return f"net.slice{s + 1}: {pool} is not MaxPool2d(2, 2)"
+        for conv, act in zip(mods[s > 0::2], mods[1 + (s > 0)::2]):
+            if not (type(conv) is nn.Conv2d and tuple(conv.kernel_size) == (3, 3) and tuple(conv.stride) == (1, 1)
+                    and tuple(conv.padding) == (1, 1) and tuple(conv.dilation) == (1, 1) and conv.groups == 1
+                    and conv.padding_mode == "zeros"):
+                return f"net.slice{s + 1}: {conv} is not a 3x3 / pad 1 / stride 1 Conv2d"
+            if (conv.in_channels, conv.out_channels) != VGG16_CONVS[ci]:
+                return f"net.slice{s + 1}: {conv} is not VGG16's conv {ci} {VGG16_CONVS[ci]}"
+            if type(act) is not nn.ReLU:
+                return f"net.slice{s + 1}: {act} after a conv is not nn.ReLU"
+            ci += 1
+    taps_c = (64, 128, 256, 512, 512)
+    for k, model in enumerate(_lin_layers(lp)):
+        mods = list(model.children()) if isinstance(model, nn.Sequential) else []
+        drop = mods[0] if len(mods) == 2 and type(mods[0]) is nn.Dropout else None
+        conv = mods[-1] if mods and len(mods) == 1 + (drop is not None) else None
+        if not (type(conv) is nn.Conv2d and tuple(conv.kernel_size) == (1, 1) and conv.bias is None
+                and conv.out_channels == 1 and conv.in_channels == taps_c[k] and conv.groups == 1):
+            return f"lin{k} is not [nn.Dropout] + a bias-free 1x1 Conv2d({taps_c[k]}, 1)"
+        if drop is not None and not 0.0 <= drop.p < 1.0:
+            return f"lin{k}: dropout p={drop.p} is not in [0, 1)"
+    return None
+
+
+def _lpips_dropout(lp: nn.Module) -> float:
+    """The dropout probability every lin_k applies now: its Dropout's p in training mode, 0 in eval mode."""
+    ps = set()
+    for model in _lin_layers(lp):
+        drop = model[0] if type(model[0]) is nn.Dropout else None
+        ps.add(float(drop.p) if drop is not None and drop.training else 0.0)
+    if len(ps) != 1:
+        raise ValueError(f"lpips: the lin layers apply different dropout probabilities {sorted(ps)}; the head draws one p")
+    return ps.pop()
+
+
+def _vgg_forward(x: torch.Tensor, lp: nn.Module, keep_all: bool):
+    """ScalingLayer + the 13 convs (ReLU fused) and the pools of one branch: (the 5 taps, every ReLU output if keep_all)."""
+    n, _, h, w = x.shape
+    sl = lp.scaling_layer
+    xs = (x.float() - sl.shift.float()) / sl.scale.float()
+    a = torch.empty(n, 1, h, w, 64, device=x.device, dtype=torch.bfloat16)
+    ops.conv3d_pack(xs.unsqueeze(2), a, t_offset=0)
+    taps, acts = [], []
+    for s, mods in enumerate(_vgg_modules(lp)):
+        if s > 0:
+            c = a.shape[-1]
+            pooled = torch.empty(n, 1, h // 2, w // 2, c, device=x.device, dtype=torch.bfloat16)
+            ops.maxpool2x2(a.view(n, h, w, c), pooled.view(n, h // 2, w // 2, c))
+            a, h, w = pooled, h // 2, w // 2
+        for conv in mods[s > 0::2]:
+            y = torch.empty(n, 1, h, w, conv.out_channels, device=x.device, dtype=torch.bfloat16)
+            ops.causal_conv3d(a, _vgg_filter(conv.weight), _vgg_bias(conv.bias), y, kernel=(1, 3, 3), relu=True)
+            a = y
+            if keep_all:
+                acts.append(y)
+        taps.append(a)
+    return taps, acts
+
+
+def _vgg_backward(acts, other_taps, lp, g, p, seed, x_shape, x_dtype):
+    """The input gradient of one branch: the slices in reverse, the tap backward at each tap, the data-gradient convs with
+    the ReLU select inside a slice, and the first conv's 3 channels in fp32, through the ScalingLayer."""
+    lins = [_lin_weight(m[-1]) for m in _lin_layers(lp)]
+    slices = _vgg_modules(lp)
+    end, d_next = len(acts), None
+    for s in reversed(range(5)):
+        convs = slices[s][s > 0::2]
+        mine = acts[end - len(convs):end]
+        n, _, h, w, c = mine[-1].shape
+        dz = torch.empty_like(mine[-1])
+        ops.lpips_tap_bwd(mine[-1].view(n, h, w, c), other_taps[s].view(n, h, w, c), lins[s], g, d_next, dz.view(n, h, w, c),
+                          tap=s, p=p, seed=seed)
+        for j in reversed(range(len(convs))):
+            wgt = _vgg_dgrad_filter(convs[j].weight)
+            if j > 0:
+                out = torch.empty_like(mine[j - 1])
+                ops.causal_conv3d(dz, wgt, None, out, kernel=(1, 3, 3), select=mine[j - 1])
+                dz = out
+            elif s > 0:
+                out = torch.empty(n, 1, h, w, convs[j].in_channels, device=dz.device, dtype=torch.bfloat16)
+                ops.causal_conv3d(dz, wgt, None, out, kernel=(1, 3, 3))
+                d_next = out.view(n, h, w, convs[j].in_channels)
+            else:
+                out = torch.empty(n, 1, h, w, 3, device=dz.device, dtype=torch.float32)
+                ops.causal_conv3d(dz, wgt, None, out, kernel=(1, 3, 3), store_channels=3)
+                dx = out.view(n, h, w, 3).permute(0, 3, 1, 2) / lp.scaling_layer.scale.float()
+        end -= len(convs)
+    return dx.to(x_dtype).reshape(x_shape)
+
+
+class _LPIPS(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x0, x1, lp, p, seed):
+        need = ctx.needs_input_grad[:2]
+        taps0, acts0 = _vgg_forward(x0, lp, need[0])
+        taps1, acts1 = _vgg_forward(x1, lp, need[1])
+        val = torch.empty(x0.shape[0], device=x0.device, dtype=torch.float32)
+        ops.lpips_head_fwd([t.view(t.shape[0], *t.shape[2:]) for t in taps0], [t.view(t.shape[0], *t.shape[2:]) for t in taps1],
+                           [_lin_weight(m[-1]) for m in _lin_layers(lp)], val, p=p, seed=seed)
+        # a branch that needs a gradient keeps every ReLU output (its taps among them), the other one its five taps;
+        # through save_for_backward, so saved-tensor hooks manage them
+        kept0 = acts0 if need[0] else taps0
+        kept1 = acts1 if need[1] else taps1
+        ctx.save_for_backward(*kept0, *kept1, *([seed] if seed is not None else []))
+        ctx.lp, ctx.p, ctx.n0, ctx.n1, ctx.has_seed = lp, p, len(kept0), len(kept1), seed is not None
+        ctx.shapes, ctx.dtypes = (x0.shape, x1.shape), (x0.dtype, x1.dtype)
+        return val.view(-1, 1, 1, 1)
+
+    @staticmethod
+    def backward(ctx, gval):
+        saved = ctx.saved_tensors
+        kept = (saved[:ctx.n0], saved[ctx.n0:ctx.n0 + ctx.n1])
+        seed = saved[-1] if ctx.has_seed else None
+        tap_at = [sum(VGG16_SLICES[:s + 1]) - 1 for s in range(5)]
+        taps = [k if len(k) == 5 else [k[i] for i in tap_at] for k in kept]
+        g = gval.reshape(-1).float().contiguous()
+        grads = [None, None]
+        for b in (0, 1):
+            if ctx.needs_input_grad[b]:
+                grads[b] = _vgg_backward(kept[b], taps[1 - b], ctx.lp, g, ctx.p, seed, ctx.shapes[b], ctx.dtypes[b])
+        return grads[0], grads[1], None, None, None
+
+
+def lpips(input: torch.Tensor, target: torch.Tensor, module: nn.Module) -> torch.Tensor:
+    """LPIPS.forward(input, target) (video_vae/modeling_lpips.py:32-45) of the reference LPIPS `module` on the library's
+    kernels: fp32 [N, 1, 1, 1].  input / target: [N, 3, H, W] bf16 or fp32, H and W multiples of 16; gradients flow to
+    either or both, in each one's dtype.  The lin layers' Dropout applies when the module is in training mode (p from the
+    module, the mask from torch's CUDA generator: torch.manual_seed reproduces it)."""
+    why = _lpips_refusal(module)
+    if why is not None:
+        raise ValueError(f"lpips: {why}")
+    if input.dim() != 4 or input.shape != target.shape or input.shape[1] != 3:
+        raise ValueError(f"lpips: input {tuple(input.shape)} and target {tuple(target.shape)} are not one [N, 3, H, W] shape")
+    if input.shape[2] % 16 or input.shape[3] % 16:
+        raise ValueError(f"lpips: H and W must be multiples of 16 (four 2x2 max-pools), got {tuple(input.shape[2:])}")
+    for t in (input, target):
+        if t.dtype not in (torch.bfloat16, torch.float32):
+            raise TypeError(f"lpips: inputs must be bf16 or fp32, got {t.dtype}")
+    if not (input.is_cuda and target.is_cuda):
+        raise RuntimeError("lpips runs on the library's CUDA kernels: input and target must be CUDA tensors (there is no "
+                           "CPU path)")
+    _require_device_once()
+    p = _lpips_dropout(module)
+    seed = torch.empty(1, device=input.device, dtype=torch.int64).random_() if p > 0 else None
+    return _LPIPS.apply(input, target, module, p, seed)
+
+
+def _patched_lpips_forward(self, input, target):
+    return lpips(input, target, self)
+
+
+def _lpips_module(obj: nn.Module) -> nn.Module:
+    """The LPIPS of a CausalVideoVAELossWrapper (.loss.perceptual_loss), an LPIPSWithDiscriminator or an LPIPS."""
+    loss = getattr(obj, "loss", None)
+    if isinstance(loss, nn.Module):
+        obj = loss
+    inner = getattr(obj, "perceptual_loss", None)
+    if isinstance(inner, nn.Module):
+        obj = inner
+    if type(obj).__name__ != "LPIPS":
+        raise ValueError("no LPIPS found: pass a reference CausalVideoVAELossWrapper, LPIPSWithDiscriminator or LPIPS")
+    return obj
+
+
+def install_training_lpips(model) -> None:
+    """Run the reference LPIPS of `model` (see _lpips_module) on `lpips`."""
+    lp = _lpips_module(model)
+    why = _lpips_refusal(lp)
+    if why is not None:
+        raise ValueError(f"install_training_lpips: {why}")
+    lp.forward = types.MethodType(_patched_lpips_forward, lp)
+    setattr(lp, _LPIPS_MARK, True)
+
+
+def uninstall_training_lpips(model) -> None:
+    lp = _lpips_module(model)
+    if lp.__dict__.pop(_LPIPS_MARK, False):
+        del lp.forward

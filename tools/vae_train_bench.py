@@ -26,6 +26,18 @@ output rounded to bf16) and of the input gradients against each other.  The
 step reports how many norm inputs / gradients causal_group_norm had to copy into a layout its kernels read.  A separate
 torch.profiler pass of the convs-only and the convs + norms steps gives the device time of torch's GroupNorm / SiLU ops
 (forward and backward) and of the conv pack kernel.
+
+LPIPS (--skip-lpips to leave it out): the recipe's generator step with the real loss -- LPIPSWithDiscriminator at the
+stage-1 weights (pixel 10, perceptual 1, KL 1e-12, disc_start 250000, so the discriminator does not run) with a synthetic
+LPIPS checkpoint from a fixed seed, in training mode (LPIPS's dropout live) -- for torch, convs + norms and convs + norms +
+LPIPS, alternating, with peak memory.  LPIPS alone at the clip shape (34 + 34 frames of 256^2: B = 2 x 17 frames per
+branch) and the image shape (8 + 8): the library's lpips against the reference module under bf16 autocast, forward and
+forward + backward (gradient to the reconstruction only, as in the loss), with peak memory and algorithmic TFLOP/s
+(2 * H * W * Cin * Cout * 9 per conv and image: forward over both branches, data gradient over one; the first conv's
+3 input channels are counted as 3, not as the 64 the kernel computes).  A separate line times the first conv alone
+(3 -> 64 channels padded to 64 -> 64) and gives its padded and real FLOP counts; a profiler pass gives each kernel family's
+device time: VGG convs (forward pass), data-gradient convs (the rest of the conv kernel's time in forward + backward),
+pool, head, tap backward and the input pack.
 """
 from __future__ import annotations
 
@@ -399,6 +411,169 @@ def profile_steps(vae) -> list:
     return rows
 
 
+# ---- LPIPS -----------------------------------------------------------------------------------------------------------
+LPIPS_SHAPES = {"clip_34+34_256": (34, 256), "images_8+8_256": (8, 256)}
+
+
+def vgg_flop(n: int, hw: int, first_cin: int = 3) -> float:
+    """Algorithmic FLOP of VGG16 features[:30] (up to relu5_3) on n images of hw x hw."""
+    total, size = 0.0, hw
+    for s, idx in enumerate(((0, 1), (2, 3), (4, 5, 6), (7, 8, 9), (10, 11, 12))):
+        if s:
+            size //= 2
+        for i in idx:
+            cin, cout = VT.VGG16_CONVS[i]
+            total += 2.0 * size * size * (first_cin if i == 0 else cin) * cout * 9
+    return n * total
+
+
+def _lpips_module(seed: int = 0):
+    from oracle.pin import ref_shim
+    ref_shim.install()
+    import io
+    import warnings
+    from tests.test_train_lpips_cpu import synthetic_lpips_state
+    buf = io.BytesIO()
+    torch.save(synthetic_lpips_state(seed), buf)
+    path = Path(__import__("tempfile").mkdtemp()) / "lpips.pth"
+    path.write_bytes(buf.getvalue())
+    loss_cls = __import__("video_vae.modeling_loss", fromlist=["LPIPSWithDiscriminator"]).LPIPSWithDiscriminator
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore")
+        loss = loss_cls(disc_start=250000, kl_weight=1e-12, pixelloss_weight=10.0, perceptual_weight=1.0,
+                        lpips_ckpt=str(path))
+    path.unlink()
+    return loss.to(DEV).train()
+
+
+def bench_lpips(iters: int, warmup: int) -> list:
+    lp = _lpips_module().perceptual_loss.train()
+    rows = []
+    for name, (n, hw) in LPIPS_SHAPES.items():
+        g = torch.Generator(device=DEV).manual_seed(n)
+        x0 = torch.rand(n, 3, hw, hw, device=DEV, generator=g) * 2 - 1
+        x1 = (x0 + 0.2 * torch.randn(n, 3, hw, hw, device=DEV, generator=g)).clamp(-1, 1)
+
+        def ours_fwd():
+            with torch.no_grad():
+                return VT.lpips(x0, x1, lp)
+
+        def ref_fwd():
+            with torch.no_grad(), torch.autocast("cuda", dtype=torch.bfloat16):
+                return lp(x0, x1)
+
+        def fwd_bwd(fn_lib):
+            def run():
+                xr = x1.clone().requires_grad_(True)
+                if fn_lib:
+                    v = VT.lpips(x0, xr, lp)
+                else:
+                    with torch.autocast("cuda", dtype=torch.bfloat16):
+                        v = lp(x0, xr)
+                v.float().sum().backward()
+                return xr.grad
+            return run
+
+        f_flop, b_flop = vgg_flop(2 * n, hw), vgg_flop(n, hw)
+        row = {"lpips": name, "images_per_branch": n}
+        for key, fn, flop in (("fwd", (ours_fwd, ref_fwd), f_flop),
+                              ("fwd_bwd", (fwd_bwd(True), fwd_bwd(False)), f_flop + b_flop)):
+            for who, f in zip(("library", "torch"), fn):
+                torch.cuda.synchronize()
+                torch.cuda.empty_cache()
+                torch.cuda.reset_peak_memory_stats()
+                base = torch.cuda.memory_allocated()
+                ms = timed(f, iters, warmup)
+                row[f"{key}_{who}_ms"] = round(ms, 3)
+                row[f"{key}_{who}_peak_gib"] = round((torch.cuda.max_memory_allocated() - base) / 2 ** 30, 2)
+                row[f"{key}_{who}_tflops"] = round(flop / ms / 1e9, 1)
+            row[f"{key}_speedup"] = round(row[f"{key}_torch_ms"] / row[f"{key}_library_ms"], 3)
+        row["algorithmic_tflop_fwd"] = round(f_flop / 1e12, 3)
+        row["algorithmic_tflop_dgrad"] = round(b_flop / 1e12, 3)
+        lp.eval()
+        with torch.no_grad(), torch.autocast("cuda", dtype=torch.bfloat16):
+            row["rel_rms_eval_value_vs_torch"] = rel_rms(VT.lpips(x0, x1, lp), lp(x0, x1))
+        lp.train()
+        rows.append(row)
+
+        # the first conv alone: 3 channels padded to 64 in the packed input
+        conv = lp.net.slice1[0]
+        xp = torch.zeros(2 * n, 1, hw, hw, 64, device=DEV, dtype=torch.bfloat16)
+        y = torch.empty(2 * n, 1, hw, hw, 64, device=DEV, dtype=torch.bfloat16)
+        wf, bias = VT._vgg_filter(conv.weight), VT._vgg_bias(conv.bias)
+        ms = timed(lambda: ops.causal_conv3d(xp, wf, bias, y, kernel=(1, 3, 3), relu=True), iters, warmup)
+        real = 2.0 * 2 * n * hw * hw * 3 * 64 * 9
+        rows.append({"lpips_first_conv": name, "images": 2 * n, "ms": round(ms, 3),
+                     "padded_tflop": round(real * 64 / 3 / 1e12, 3), "real_tflop": round(real / 1e12, 4),
+                     "padded_work_over_real": round(64 / 3, 1), "padded_tflops": round(real * 64 / 3 / ms / 1e9, 1)})
+
+        fams = {"conv3d_wgmma_kernel": 0.0, "maxpool2x2_kernel": 0.0, "lpips_head": 0.0, "lpips_tap_bwd_kernel": 0.0,
+                "conv_pack_kernel": 0.0}
+        f_only = kernel_ms(ours_fwd, list(fams))
+        both = kernel_ms(fwd_bwd(True), list(fams))
+        rows.append({"lpips_profile": name, "vgg_convs_fwd_ms": round(f_only["conv3d_wgmma_kernel"], 3),
+                     "dgrad_convs_ms": round(both["conv3d_wgmma_kernel"] - f_only["conv3d_wgmma_kernel"], 3),
+                     "pool_ms": round(both["maxpool2x2_kernel"], 3), "head_fwd_ms": round(both["lpips_head"], 3),
+                     "tap_bwd_ms": round(both["lpips_tap_bwd_kernel"], 3), "input_pack_ms": round(both["conv_pack_kernel"], 3)})
+        del x0, x1, xp, y
+        torch.cuda.empty_cache()
+    return rows
+
+
+LOSS_VARIANTS = {"torch": (), "library_norms": (VT.install_training_convs, VT.install_training_norms),
+                 "library_norms_lpips": (VT.install_training_convs, VT.install_training_norms, VT.install_training_lpips)}
+
+
+def bench_step_lpips(vae, rounds: int, iters: int, warmup: int) -> list:
+    """The generator step with LPIPSWithDiscriminator (optimizer_idx 0, before disc_start)."""
+    class Step(torch.nn.Module):
+        def __init__(self):
+            super().__init__()
+            self.vae, self.loss = vae, _lpips_module()
+
+    model = Step().train()
+    params = list(model.parameters())
+
+    def step(x):
+        for p in params:
+            p.grad = None
+        with torch.autocast("cuda", dtype=torch.bfloat16):
+            posterior, dec = vae(x, sample_posterior=True, generator=torch.Generator().manual_seed(0))
+            loss, _ = model.loss(x, dec, posterior, optimizer_idx=0, global_step=0, last_layer=vae.get_last_layer())
+        loss.backward()
+        return loss
+
+    rows = []
+    for name, shape in STEP_INPUTS.items():
+        x = torch.rand(*shape, device=DEV) * 2 - 1
+        res = {v: [] for v in LOSS_VARIANTS}
+        peak, losses = {}, {}
+        for _ in range(rounds):
+            for variant, installs in LOSS_VARIANTS.items():
+                for inst in installs:
+                    inst(model)
+                try:
+                    torch.cuda.synchronize()
+                    torch.cuda.reset_peak_memory_stats()
+                    res[variant].append(timed(lambda: step(x), iters, warmup))
+                    peak[variant] = max(peak.get(variant, 0), torch.cuda.max_memory_allocated())
+                    losses[variant] = step(x).item()
+                finally:
+                    VT.uninstall_training_lpips(model)
+                    _uninstall_all(vae)
+        med = {v: statistics.median(res[v]) for v in LOSS_VARIANTS}
+        rows.append({"step_with_lpips_loss": name, **{f"{v}_ms": round(med[v], 2) for v in LOSS_VARIANTS},
+                     "speedup_norms": round(med["torch"] / med["library_norms"], 3),
+                     "speedup_norms_lpips": round(med["torch"] / med["library_norms_lpips"], 3),
+                     **{f"{v}_rounds_ms": [round(t, 2) for t in res[v]] for v in LOSS_VARIANTS},
+                     **{f"{v}_peak_gib": round(peak[v] / 2 ** 30, 2) for v in LOSS_VARIANTS},
+                     **{f"loss_{v}": losses[v] for v in LOSS_VARIANTS},
+                     "note": "pixel 10 + LPIPS 1 (dropout live) + KL 1e-12; the discriminator starts at step 250000"})
+        del x
+        torch.cuda.empty_cache()
+    return rows
+
+
 def main() -> None:
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--iters", type=int, default=10)
@@ -409,6 +584,7 @@ def main() -> None:
     ap.add_argument("--skip-families", action="store_true")
     ap.add_argument("--skip-norms", action="store_true")
     ap.add_argument("--skip-profile", action="store_true")
+    ap.add_argument("--skip-lpips", action="store_true")
     args = ap.parse_args()
     _lib.require_device()
     print(json.dumps(device_info()), flush=True)
@@ -417,13 +593,20 @@ def main() -> None:
             for row in bench_family(*fam, iters=args.iters, warmup=args.warmup):
                 print(json.dumps(row), flush=True)
             torch.cuda.empty_cache()
-    vae = None if (args.skip_step and args.skip_norms and args.skip_profile) else _reference_vae()
+    if not args.skip_lpips:
+        for row in bench_lpips(args.iters, args.warmup):
+            print(json.dumps(row), flush=True)
+        torch.cuda.empty_cache()
+    vae = None if (args.skip_step and args.skip_norms and args.skip_profile and args.skip_lpips) else _reference_vae()
     if not args.skip_norms:
         for key, names in sorted(norm_sites(vae).items(), key=lambda kv: -kv[0][0][1]):
             print(json.dumps(bench_norm_family(key, names, args.iters, args.warmup)), flush=True)
             torch.cuda.empty_cache()
     if not args.skip_step:
         for row in bench_step(vae, args.rounds, args.step_iters, 1):
+            print(json.dumps(row), flush=True)
+    if not args.skip_lpips:
+        for row in bench_step_lpips(vae, args.rounds, args.step_iters, 1):
             print(json.dumps(row), flush=True)
     if not args.skip_profile:
         for row in profile_steps(vae):
