@@ -344,6 +344,11 @@ int pf_ln_modulate(const float* x, void* y, int32_t batches, int32_t rows_per_ba
   PF_REQUIRE(dim % 128 == 0 && dim <= 128 * LN_MAX_VEC, "pf_ln_modulate: dim=%d must be a multiple of 128 and <= %d", dim, 128 * LN_MAX_VEC);
   PF_REQUIRE(batches > 0 && row_count > 0 && row_begin >= 0 && row_begin + row_count <= rows_per_batch, "pf_ln_modulate: bad row range");
   PF_REQUIRE(mod_batch_stride % 4 == 0, "pf_ln_modulate: modulation stride must be a multiple of 4 floats");
+  // float4 loads of x, shift and scale; 8-byte stores of four bf16
+  PF_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "pf_ln_modulate: x must be 16-byte aligned");
+  PF_REQUIRE((reinterpret_cast<uintptr_t>(shift) & 15) == 0, "pf_ln_modulate: shift must be 16-byte aligned");
+  PF_REQUIRE((reinterpret_cast<uintptr_t>(scale) & 15) == 0, "pf_ln_modulate: scale must be 16-byte aligned");
+  PF_REQUIRE((reinterpret_cast<uintptr_t>(y) & 7) == 0, "pf_ln_modulate: y must be 8-byte aligned");
   const long long warps = static_cast<long long>(batches) * row_count;
   const int blocks = static_cast<int>((warps + 7) / 8);
   ln_modulate_kernel<false><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -359,6 +364,12 @@ int pf_ln_modulate_fp8(const float* x, void* y, float* row_scale, int32_t batche
   PF_REQUIRE(dim % 128 == 0 && dim <= 128 * LN_MAX_VEC, "pf_ln_modulate_fp8: dim=%d must be a multiple of 128 and <= %d", dim, 128 * LN_MAX_VEC);
   PF_REQUIRE(batches > 0 && row_count > 0 && row_begin >= 0 && row_begin + row_count <= rows_per_batch, "pf_ln_modulate_fp8: bad row range");
   PF_REQUIRE(mod_batch_stride % 4 == 0, "pf_ln_modulate_fp8: modulation stride must be a multiple of 4 floats");
+  // float4 loads of x, shift and scale; 4-byte stores of four e4m3
+  PF_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "pf_ln_modulate_fp8: x must be 16-byte aligned");
+  PF_REQUIRE((reinterpret_cast<uintptr_t>(shift) & 15) == 0, "pf_ln_modulate_fp8: shift must be 16-byte aligned");
+  PF_REQUIRE((reinterpret_cast<uintptr_t>(scale) & 15) == 0, "pf_ln_modulate_fp8: scale must be 16-byte aligned");
+  PF_REQUIRE((reinterpret_cast<uintptr_t>(y) & 3) == 0, "pf_ln_modulate_fp8: y must be 4-byte aligned");
+  PF_REQUIRE((reinterpret_cast<uintptr_t>(row_scale) & 3) == 0, "pf_ln_modulate_fp8: row_scale must be 4-byte aligned");
   const long long warps = static_cast<long long>(batches) * row_count;
   const int blocks = static_cast<int>((warps + 7) / 8);
   ln_modulate_kernel<true><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -394,8 +405,10 @@ int pf_small_linear(const float* x, int32_t m, int32_t k, const void* w, const f
   PF_REQUIRE(x && w && y, "pf_small_linear: null pointer");
   PF_REQUIRE(m >= 1 && m <= SL_MAX_M, "pf_small_linear: m=%d must be in [1, %d]", m, SL_MAX_M);
   PF_REQUIRE(k % 8 == 0 && k > 0, "pf_small_linear: k=%d must be a multiple of 8", k);
+  PF_REQUIRE(n > 0, "pf_small_linear: n=%d must be positive", n);
+  PF_REQUIRE(4LL * m * k <= 96 * 1024, "pf_small_linear: m*k too large for shared memory");
   const int smem = m * k * 4;
-  PF_REQUIRE(smem <= 96 * 1024, "pf_small_linear: m*k too large for shared memory");
+  PF_REQUIRE((reinterpret_cast<uintptr_t>(w) & 15) == 0, "pf_small_linear: w must be 16-byte aligned (16-byte loads)");
   const int blocks = (n + 7) / 8;
 #define PF_SL_CASE(MM)                                                                                          \
   case MM: {                                                                                                    \
@@ -433,7 +446,9 @@ int pf_patchify(const void* latent, int32_t latent_is_f32, int32_t b, int32_t c,
   using namespace pf;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   PF_REQUIRE(latent && tokens && h % 2 == 0 && w % 2 == 0, "pf_patchify: bad arguments");
-  PF_REQUIRE(tok_begin >= 0 && tok_begin + t * (h / 2) * (w / 2) <= rows_per_batch, "pf_patchify: token range exceeds rows_per_batch");
+  PF_REQUIRE(b > 0 && c > 0 && t > 0 && h > 0 && w > 0, "pf_patchify: b=%d c=%d t=%d h=%d w=%d must be positive", b, c, t, h, w);
+  PF_REQUIRE(tok_begin >= 0 && tok_begin + static_cast<long long>(t) * (h / 2) * (w / 2) <= rows_per_batch,
+             "pf_patchify: token range exceeds rows_per_batch");
   const long long total = static_cast<long long>(b) * c * t * h * w;
   const int blocks = static_cast<int>((total + 255) / 256);
   if (latent_is_f32)
@@ -451,6 +466,10 @@ int pf_unpatchify(const float* x, int32_t rows_per_batch, int32_t row_begin, int
   using namespace pf;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   PF_REQUIRE(x && out && h % 2 == 0 && w % 2 == 0, "pf_unpatchify: bad arguments");
+  PF_REQUIRE(b > 0 && c > 0 && t > 0 && h > 0 && w > 0, "pf_unpatchify: b=%d c=%d t=%d h=%d w=%d must be positive", b, c, t, h, w);
+  PF_REQUIRE(row_begin >= 0, "pf_unpatchify: row_begin=%d must be >= 0", row_begin);
+  PF_REQUIRE(row_begin + static_cast<long long>(t) * (h / 2) * (w / 2) <= rows_per_batch,
+             "pf_unpatchify: token range [row_begin %d, +t*(h/2)*(w/2)) exceeds rows_per_batch %d", row_begin, rows_per_batch);
   const long long total = static_cast<long long>(b) * c * t * h * w;
   const int blocks = static_cast<int>((total + 255) / 256);
   if (out_is_f32)

@@ -310,6 +310,10 @@ int pf_rms_norm_rows(const float* x, void* y, const float* w, int32_t batches, i
   using namespace pf;
   PF_REQUIRE(x && y && w, "pf_rms_norm_rows: null pointer");
   PF_REQUIRE(dim > 0 && dim % 4 == 0, "pf_rms_norm_rows: dim=%d must be a positive multiple of 4", dim);
+  // float4 loads of x and w; 8-byte stores of four bf16
+  PF_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "pf_rms_norm_rows: x must be 16-byte aligned");
+  PF_REQUIRE((reinterpret_cast<uintptr_t>(w) & 15) == 0, "pf_rms_norm_rows: w must be 16-byte aligned");
+  PF_REQUIRE((reinterpret_cast<uintptr_t>(y) & 7) == 0, "pf_rms_norm_rows: y must be 8-byte aligned");
   PF_REQUIRE(batches > 0 && row_count > 0 && row_begin >= 0 && row_begin + row_count <= rows_per_batch,
              "pf_rms_norm_rows: bad row range (batches %d rows %d begin %d count %d)", batches, rows_per_batch, row_begin, row_count);
   const long long warps = static_cast<long long>(batches) * row_count;
